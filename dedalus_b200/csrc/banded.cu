@@ -30,9 +30,13 @@ __device__ __forceinline__ bool bd_finite(double v) { return v - v == 0.0; }
 //   bit 0: the factor kernel re-reads band entries that other lanes wrote with L2 loads (ld.global.cg) behind a CTA fence
 //          instead of relying on the SM's L1 for lane-to-lane communication through global memory;
 //   bit 1: the solve kernel reads the factor columns straight from global memory instead of through the cp.async ring.
-// One verification of variant 0 in a fresh process once came back with a backward error of 1.2e-5 and could not be
-// reproduced -- until that is understood the variant without asynchronous copies is the default and every factorisation is
-// verified (and retried) by dedalus_b200/sphere.py SphereSystems.factor_verified.
+// A backward error of 1.2e-5 seen once from variant 0 is explained by a race in the solve's cp.async ring: when its prologues
+// committed fewer than BS_DEPTH - 1 groups (n < BS_DEPTH - 1; n = 2 NC = 6 for the m = Lmax system of the stock shallow-water
+// problem), the wait of step j did not cover column j, so the forward sweep could read L columns that had not landed and the
+// backward sweep a ring slot still holding a forward-sweep column.  tests/test_emu_banded.py, where emulated copies land only
+// when their group is retired, checks every variant at those sizes.  Whether the ring solve is faster has not been measured, so
+// the variant without asynchronous copies stays the default, and dedalus_b200/sphere.py SphereSystems.factor_verified still
+// verifies (and retries) every factorisation.
 static int g_bd_mode = -1;
 static int bd_mode()
 {
@@ -183,8 +187,11 @@ k_banded_solve(const db_banded_sys* __restrict__ sys, int kl, int ku, const doub
     }
     for (int i = lane; i < n; i += 32) piv[i] = ipiv_all[S.piv_off + i] - i;
     // ---- forward sweep: y = L^{-1} P b
-    for (int d = 0; d < BS_DEPTH - 1 && d < n && !direct; ++d) {
-        for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[d * ldf + l], &ab[(int64_t)d * ldf + l]);
+    // Both prologues commit exactly BS_DEPTH - 1 groups, empty ones past the last column, so that group j always holds column j
+    // and the wait of step j (all but the BS_DEPTH - 1 newest groups) covers it for every n.
+    for (int d = 0; d < BS_DEPTH - 1 && !direct; ++d) {
+        if (d < n)
+            for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[d * ldf + l], &ab[(int64_t)d * ldf + l]);
         db_cp_commit();
     }
     DB_WARP_SYNC();
@@ -213,9 +220,9 @@ k_banded_solve(const db_banded_sys* __restrict__ sys, int kl, int ku, const doub
     // ---- backward sweep: x = U^{-1} y  (column oriented: x_j = y_j / U_jj, then y_i -= U_ij x_j for i = j - kv .. j - 1)
     db_cp_wait<0>();
     DB_WARP_SYNC();
-    for (int d = 0; d < BS_DEPTH - 1 && d < n && !direct; ++d) {
-        const int c = n - 1 - d;
-        for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[d * ldf + l], &ab[(int64_t)c * ldf + l]);
+    for (int d = 0; d < BS_DEPTH - 1 && !direct; ++d) {
+        if (d < n)
+            for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[d * ldf + l], &ab[(int64_t)(n - 1 - d) * ldf + l]);
         db_cp_commit();
     }
     DB_WARP_SYNC();

@@ -23,11 +23,12 @@
 
 // asynchronous global -> shared copies (LDGSTS) used for deep software prefetch without register cost
 #ifdef DB_EMU
-__device__ __forceinline__ void db_cp_async8(void* dst, const void* src) { *reinterpret_cast<double*>(dst) = *reinterpret_cast<const double*>(src); }
-__device__ __forceinline__ void db_cp_async4(void* dst, const void* src) { *reinterpret_cast<int*>(dst) = *reinterpret_cast<const int*>(src); }
-__device__ __forceinline__ void db_cp_async16(void* dst, const void* src) { memcpy(dst, src, 16); }
-__device__ __forceinline__ void db_cp_commit() {}
-template <int N> __device__ __forceinline__ void db_cp_wait() {}
+// (the emulation defers each copy until a wait retires its group: tests/emu/cuda_emu.h)
+__device__ __forceinline__ void db_cp_async8(void* dst, const void* src) { emu_cp_async(dst, src, 8); }
+__device__ __forceinline__ void db_cp_async4(void* dst, const void* src) { emu_cp_async(dst, src, 4); }
+__device__ __forceinline__ void db_cp_async16(void* dst, const void* src) { emu_cp_async(dst, src, 16); }
+__device__ __forceinline__ void db_cp_commit() { emu_cp_commit(); }
+template <int N> __device__ __forceinline__ void db_cp_wait() { emu_cp_wait(N); }
 #else
 __device__ __forceinline__ void db_cp_async8(void* dst, const void* src)
 {

@@ -331,7 +331,8 @@ int db_banded_solve(const db_banded_sys* sys, int32_t nsys, int32_t kl, int32_t 
 int db_banded_matvec(const db_banded_sys* sys, int32_t nsys, int32_t kl, int32_t ku, const double* a_ab, const double* b_ab,
                      const double* x, double* ya, double* yb, void* stream);
 /* diagnostic variants of the two kernels above (also environment DB_BANDED_MODE): bit 0 = the factorisation re-reads entries
- * written by other lanes through L2 behind a CTA fence, bit 1 = the solve reads factor columns directly from global memory */
+ * written by other lanes through L2 behind a CTA fence, bit 1 = the solve reads factor columns directly from global memory;
+ * a negative mode returns to DB_BANDED_MODE (default 3) */
 int db_banded_set_mode(int32_t mode);
 /* gather (vec[e] = idx[e] >= 0 ? arena[idx[e]] : 0) / scatter (arena[idx[e]] = vec[e] where idx[e] >= 0) through an index
  * table: pencil vectors <-> coefficient arrays in the folded triangular (m, l) packing (core/subsystems.py:340-371) */

@@ -80,6 +80,52 @@ double emu_shfl_exchange(double v, int src_lane) {
     return shfl_slots[p][(tid & ~31u) + (unsigned)src_lane];
 }
 
+// cp.async: one queue per thread slot of the running block.  A copy belongs to the open group (numbered by the count of groups
+// committed before it); cp.async.wait_group n lands, in issue order, the copies of every group but the n most recent.  The source is
+// read at landing time too: the kernels never write what they prefetch while the copy is in flight.
+namespace {
+struct CpCopy { void* dst; const void* src; size_t bytes; size_t group; };
+struct CpQueue {
+    std::vector<CpCopy> copies;
+    size_t head = 0, committed = 0;
+    void reset() { copies.clear(); head = 0; committed = 0; }
+};
+thread_local CpQueue cp_queues[1024];
+bool cp_late() {
+    static const bool late = [] {
+        const char* e = getenv("DB_EMU_CP");
+        if (!e || !strcmp(e, "late")) return true;
+        if (!strcmp(e, "early")) return false;
+        fprintf(stderr, "DB_EMU_CP=%s: expected 'late' or 'early'\n", e);
+        abort();
+    }();
+    return late;
+}
+CpQueue& cp_queue() {
+    const EmuState& s = emu_cur;
+    return cp_queues[s.tid.x + s.bdim.x * (s.tid.y + s.bdim.y * s.tid.z)];
+}
+}  // namespace
+
+void emu_cp_async(void* dst, const void* src, size_t bytes) {
+    if (!cp_late()) { std::memcpy(dst, src, bytes); return; }
+    CpQueue& q = cp_queue();
+    q.copies.push_back({dst, src, bytes, q.committed});
+}
+
+void emu_cp_commit() { ++cp_queue().committed; }
+
+void emu_cp_wait(int n) {
+    CpQueue& q = cp_queue();
+    if (q.committed <= (size_t)n) return;
+    const size_t retire = q.committed - (size_t)n;        // groups 0 .. retire - 1 complete
+    while (q.head < q.copies.size() && q.copies[q.head].group < retire) {
+        const CpCopy& c = q.copies[q.head++];
+        std::memcpy(c.dst, c.src, c.bytes);
+    }
+    if (q.head == q.copies.size()) { q.copies.clear(); q.head = 0; }
+}
+
 void emu_launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>& body) {
     const size_t nthreads = (size_t)block.x * block.y * block.z;
     // the launch limits of the real device (sm_90): a launch that violates them fails on the GPU with "invalid configuration
@@ -102,6 +148,8 @@ void emu_launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>&
                        bx = reverse_blocks ? grid.x - 1 - bxi : bxi;
         std::memset(shared.data(), 0xA5, shared.size());   // poison shared memory
         std::memset(shfl_parity, 0, sizeof(shfl_parity));
+        // copies still pending when a thread of the previous block exited never land in this block's shared memory
+        for (size_t t = 0; t < nthreads; ++t) cp_queues[t].reset();
         size_t i = 0;
         for (unsigned tz = 0; tz < block.z; ++tz)
         for (unsigned ty = 0; ty < block.y; ++ty)

@@ -67,6 +67,13 @@ static inline int atomicAdd(int* p, int v) { int o = *p; *p += v; return o; }
 static inline int atomicMax(int* p, int v) { int o = *p; if (v > o) *p = v; return o; }
 static inline int atomicOr(int* p, int v) { int o = *p; *p |= v; return o; }
 
+// asynchronous global -> shared copies (cp.async): each thread keeps its own queue of committed groups.  With DB_EMU_CP=late (the
+// default) a copy lands only when a wait retires its group, so shared memory read before that still holds the 0xA5 poison (or an
+// older value); with DB_EMU_CP=early it lands at issue, so a slot refilled while other code still reads it shows the new value.
+void emu_cp_async(void* dst, const void* src, size_t bytes);
+void emu_cp_commit();                // close the open group (also when it is empty), as cp.async.commit_group
+void emu_cp_wait(int n);             // land every committed group except the n most recent, as cp.async.wait_group n
+
 void emu_launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>& body);
 
 #define DB_LAUNCH(kern, grid, block, smem, stream, ...) \
