@@ -165,13 +165,223 @@ __device__ __forceinline__ void twiddle_odd_half(double2 (&o)[N], std::integer_s
     ((void)(o[M] = mul_tw<M, 2 * N, INV>(o[M])), ...);
 }
 
-// u[b] = lo[b] + W3^(2c) hi[b], then * W_NA^(b c)      (backward stage A, residue C)
-template <int C, int Q, bool INV>
-__device__ __forceinline__ void residue_combine(double2 (&u)[Q], const double2 (&lo)[Q], const double2 (&hi)[Q])
+// forward stage 2, residue C of the outputs: t[b] = sum_a' W3^(a' C) B[Q a' + b], times W_NA^(b C)
+template <int C, int Q>
+__device__ __forceinline__ void residue_gather(double2 (&u)[Q], const double2* src, int stride)
 {
 #pragma unroll
-    for (int b = 0; b < Q; ++b) u[b] = cadd2(lo[b], mul_tw<(2 * C) % 3, 3, INV>(hi[b]));
-    twiddle_row<C, 3 * Q, INV>(u, std::make_integer_sequence<int, Q>{});
+    for (int b = 0; b < Q; ++b) {
+        const double2 b0 = src[b * stride], b1 = src[(Q + b) * stride], b2 = src[(2 * Q + b) * stride];
+        u[b] = cadd2(b0, cadd2(mul_tw<C % 3, 3, false>(b1), mul_tw<(2 * C) % 3, 3, false>(b2)));
+    }
+    twiddle_row<C, 3 * Q, false>(u, std::make_integer_sequence<int, Q>{});
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// The register stages of the x passes, shared by k_rbwd_regs / k_rfwd_regs and the fused k_rfft_x_products.
+// Roles of thread (p, r): p = line pair of the tile, r = threadIdx.x / P (see RegGeom).
+// ---------------------------------------------------------------------------------------------------------
+
+// backward, load + stage A: spectrum of the staged coefficient rows `in` ([M][P] double2: row 2k = re, 2k+1 = im of mode k
+// for both lines of every pair) with (i k kscale)^deriv applied, then this thread's residue of the size-NA DFT (threads r < 3 NB)
+template <int Q, int NB, bool DERIV>
+__device__ __forceinline__ void rbwd_load_a(const double2* in, int p, int r, int M, int deriv_, double kscale, double2 (&u)[Q])
+{
+    constexpr int P = RR_P;
+    const int Kmax = (M - 1) / 2;
+    const int deriv = DERIV ? deriv_ : 0;
+    // (i k kscale)^deriv = (ur + i ui) (k kscale)^deriv
+    const double ur = ((deriv & 3) == 0) ? 1.0 : ((deriv & 3) == 2) ? -1.0 : 0.0;
+    const double ui = ((deriv & 3) == 1) ? 1.0 : ((deriv & 3) == 3) ? -1.0 : 0.0;
+    const int n2 = r % NB, c = r / NB;
+    // Z_k = X1_k + i X2_k (k <= Kmax), Z_{n-k} = conj X1_k + i conj X2_k, X_k = (c_2k + i c_2k+1) / 2, X_0 = c_0
+    auto spec = [&](int k, bool mirrored) -> double2 {
+        if (k > Kmax) return make_double2(0.0, 0.0);
+        const double2 R = in[(2 * k) * P + p];                      // (re line 1, re line 2)
+        if (k == 0) return DERIV ? make_double2(0.0, 0.0) : R;
+        const double2 I = in[(2 * k + 1) * P + p];                  // (im line 1, im line 2)
+        if (DERIV) {
+            const double ks = kscale * k, ks2 = ks * ks;
+            const double f = 0.5 * ((deriv == 1) ? ks : (deriv == 2) ? ks2 : (deriv == 3) ? ks2 * ks : ks2 * ks2);
+            const double mr = ur * f, mi = ui * f;
+            const double2 R2 = make_double2(mr * R.x - mi * I.x, mr * R.y - mi * I.y);
+            const double2 I2 = make_double2(mi * R.x + mr * I.x, mi * R.y + mr * I.y);
+            return mirrored ? make_double2(R2.x + I2.y, R2.y - I2.x) : make_double2(R2.x - I2.y, I2.x + R2.y);
+        }
+        return mirrored ? make_double2(0.5 * (R.x + I.y), 0.5 * (R.y - I.x)) : make_double2(0.5 * (R.x - I.y), 0.5 * (I.x + R.y));
+    };
+    // stage A: size-NA DFT over n1 = Q a + b with the a = 1 third identically zero; this thread's residue c:
+    // u[b] = Z[NB b + n2] + W3^(2c) Z[NB (2Q + b) + n2], times W_NA^(b c), each pair of modes combined as soon as it is loaded
+    // (the spectrum is never held in registers as a whole)
+    double2 lo[Q], hi[Q];
+#pragma unroll
+    for (int b = 0; b < Q; ++b) {
+        lo[b] = spec(NB * b + n2, false);
+        hi[b] = spec(NB * (Q - b) - n2, true);
+    }
+    auto combine = [&](auto CC) {
+        constexpr int C = decltype(CC)::value;
+#pragma unroll
+        for (int b = 0; b < Q; ++b) u[b] = cadd2(lo[b], mul_tw<(2 * C) % 3, 3, true>(hi[b]));
+        twiddle_row<C, 3 * Q, true>(u, std::make_integer_sequence<int, Q>{});
+    };
+    if (c == 0) combine(std::integral_constant<int, 0>{});
+    else if (c == 1) combine(std::integral_constant<int, 1>{});
+    else combine(std::integral_constant<int, 2>{});
+}
+
+// backward, end of stage A: radix-2 part and twiddle, stored to the exchange buffer ([N][P] double2, threads r < 3 NB)
+template <int Q, int NB>
+__device__ __forceinline__ void rbwd_exchange_a(double2 (&u)[Q], double2* xch, const double* __restrict__ tw, int p, int r)
+{
+    constexpr int P = RR_P;
+    const int n2 = r % NB, c = r / NB;
+    DftP2<Q, true>::run(u);
+    double2* dst = xch + n2 * P + p;
+#pragma unroll
+    for (int kb = 0; kb < Q; ++kb) {
+        const int kk = 3 * kb + c;                         // output k1
+        dst[kk * NB * P] = cmulc2(u[kb], ldtwn(tw, n2 * kk));
+    }
+}
+
+// backward stage B (threads r < 6 Q): size-NB DFT over n2 for fixed k1 = r % NA, outputs k2 = 2 m + h (h = r / NA), so v[m] is
+// the pair's grid value at j = k1 + NA (2 m + h)
+template <int Q, int NB>
+__device__ __forceinline__ void rbwd_stage_b(const double2* xch, int p, int r, double2 (&v)[NB / 2])
+{
+    constexpr int P = RR_P, NA = 3 * Q, H = NB / 2;
+    const int k1 = r % NA, h = r / NA;
+    const double2* src = xch + (k1 * NB) * P + p;
+    if (h == 0) {
+#pragma unroll
+        for (int m = 0; m < H; ++m) v[m] = cadd2(src[m * P], src[(m + H) * P]);
+    } else {
+#pragma unroll
+        for (int m = 0; m < H; ++m) v[m] = csub2(src[m * P], src[(m + H) * P]);
+        twiddle_odd_half<true>(v, std::make_integer_sequence<int, H>{});
+    }
+    DftP2<H, true>::run(v);
+}
+
+// forward stage 1 load (threads r < 6 Q): first radix-2 split (DIF) of the size-NB DFT over j2 for fixed j1 = r % NA of the staged
+// grid rows `in` ([N][P] double2, grid index j = j1 + NA j2)
+template <int Q, int NB>
+__device__ __forceinline__ void rfwd_load_1(const double2* in, int p, int r, double2 (&v)[NB / 2])
+{
+    constexpr int P = RR_P, NA = 3 * Q, H = NB / 2;
+    const int j1 = r % NA, h = r / NA;
+    const double2* src = in + j1 * P + p;
+    if (h == 0) {
+#pragma unroll
+        for (int m = 0; m < H; ++m) v[m] = cadd2(src[(NA * m) * P], src[(NA * (m + H)) * P]);
+    } else {
+#pragma unroll
+        for (int m = 0; m < H; ++m) v[m] = csub2(src[(NA * m) * P], src[(NA * (m + H)) * P]);
+        twiddle_odd_half<false>(v, std::make_integer_sequence<int, H>{});
+    }
+}
+
+// forward, end of stage 1: the rest of the size-NB DFT and the twiddle, stored to the exchange buffer
+template <int Q, int NB>
+__device__ __forceinline__ void rfwd_exchange_1(double2 (&v)[NB / 2], double2* xch, const double* __restrict__ tw, int p, int r)
+{
+    constexpr int P = RR_P, NA = 3 * Q, H = NB / 2;
+    const int j1 = r % NA, h = r / NA;
+    DftP2<H, false>::run(v);
+    double2* dst = xch + (j1 * NB + h) * P + p;
+#pragma unroll
+    for (int m = 0; m < H; ++m) {
+        const int kk = 2 * m + h;                          // output k2
+        dst[(2 * m) * P] = (kk == 0) ? v[m] : cmul2(v[m], ldtwn(tw, j1 * kk));
+    }
+}
+
+// forward stage 2 (threads r < 3 NB): size-NA DFT over j1 = Q a' + b for fixed k2 = r % NB; this thread's output residue
+// c = r / NB: z[kb] is mode k1 = c + 3 kb
+template <int Q, int NB>
+__device__ __forceinline__ void rfwd_stage_2(const double2* xch, int p, int r, double2 (&z)[Q])
+{
+    constexpr int P = RR_P;
+    const int k2 = r % NB, c = r / NB;
+    const double2* src = xch + k2 * P + p;
+    if (c == 0) residue_gather<0, Q>(z, src, NB * P);
+    else if (c == 1) residue_gather<1, Q>(z, src, NB * P);
+    else residue_gather<2, Q>(z, src, NB * P);
+    DftP2<Q, false>::run(z);
+}
+
+// forward: park the high third (k1 >= 2Q) as Zhi[k1 - 2Q][k2] for the mirror partners
+template <int Q, int NB>
+__device__ __forceinline__ void rfwd_park(const double2 (&z)[Q], double2* xch, int p, int r)
+{
+    constexpr int P = RR_P;
+    const int k2 = r % NB, c = r / NB;
+    double2* dst = xch + k2 * P + p;
+#pragma unroll
+    for (int kb = 0; kb < Q; ++kb) {
+        const int kk = 3 * kb + c;
+        if (kk >= 2 * Q) dst[(kk - 2 * Q) * NB * P] = z[kb];
+    }
+}
+
+// forward: the two real lines' cos / -sin coefficients of every mode k <= Kmax this thread owns, scaled, stored to rows 2k, 2k+1
+template <int Q, int NB>
+__device__ __forceinline__ void rfwd_store(const double2 (&z)[Q], const double2* xch, int p, int r, const RegArgs& a, double* gout,
+                                           int64_t o)
+{
+    constexpr int P = RR_P, N = 3 * Q * NB;
+    const int k2 = r % NB, c = r / NB;
+    const int M = a.M, Kmax = (a.M - 1) / 2;
+    const int64_t inner = a.inner;
+    // Z_{n-k} for k = NB k1 + k2 sits at Zhi[(Q - 1 - k1), NB - k2] for k2 > 0, Zhi[Q - k1, 0] for k2 = 0
+    const double sc = 1.0 / N;
+    const int k2p = (k2 == 0) ? 0 : NB - k2;
+    const double2* src = xch + k2p * P + p;
+#pragma unroll
+    for (int kb = 0; kb < Q; ++kb) {
+        const int kk = 3 * kb + c;                         // k1
+        const int k = NB * kk + k2;
+        if (kk >= Q || k > Kmax) continue;
+        double* row = out_row_ptr(a, gout, o, 2 * k, M, inner);
+        double* row1 = out_row_ptr(a, gout, o, 2 * k + 1, M, inner);
+        const double2 za = z[kb];
+        if (k == 0) {
+            *reinterpret_cast<double2*>(row) = make_double2(za.x * sc, za.y * sc);
+            *reinterpret_cast<double2*>(row1) = make_double2(0.0, 0.0);
+        } else {
+            const int kbp = (k2 == 0) ? Q - kk : Q - 1 - kk;
+            const double2 zb = src[kbp * NB * P];
+            *reinterpret_cast<double2*>(row) = make_double2((za.x + zb.x) * sc, (za.y + zb.y) * sc);
+            *reinterpret_cast<double2*>(row1) = make_double2((za.y - zb.y) * sc, (zb.x - za.x) * sc);
+        }
+    }
+}
+
+struct OutCol { double* g; int64_t o; };       // a pair's column in the output rows, outer index
+
+// the whole forward transform of the grid tile staged in `buf` ([N][P] double2), which is also its exchange buffer; every
+// thread of the CTA calls it (it contains barriers), and `buf` may be overwritten once the caller has passed a barrier after it.
+// dest() -> (this pair's column in the output rows, outer index) is evaluated only at the store.
+template <int Q, int NB, class Dest>
+__device__ __forceinline__ void rfwd_tile(double2* buf, int p, int r, const RegArgs& a, Dest dest)
+{
+    constexpr int NA = 3 * Q, H = NB / 2;
+    const bool in_1 = r < 2 * NA, in_2 = r < 3 * NB;
+    double2 v[H];
+    if (in_1) rfwd_load_1<Q, NB>(buf, p, r, v);
+    __syncthreads();                                           // inputs are consumed: reuse `buf` as exchange
+    if (in_1) rfwd_exchange_1<Q, NB>(v, buf, a.twn, p, r);
+    __syncthreads();
+    double2 z[Q];
+    if (in_2) rfwd_stage_2<Q, NB>(buf, p, r, z);
+    __syncthreads();
+    if (in_2) rfwd_park<Q, NB>(z, buf, p, r);
+    __syncthreads();
+    if (in_2) {
+        const auto d = dest();
+        rfwd_store<Q, NB>(z, buf, p, r, a, d.g, d.o);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -186,16 +396,10 @@ k_rbwd_regs(RegArgs a, TileWalk tw_)
     DB_SMEM(double2, sm);                                   // 2 buffers of [N][P] double2
     const int p = threadIdx.x & (P - 1), r = threadIdx.x >> 3;
     const int64_t inner = a.inner;
-    const int M = a.M, Kmax = (a.M - 1) / 2;
-    const int deriv = DERIV ? a.deriv : 0;
-    // (i k kscale)^deriv = (ur + i ui) (k kscale)^deriv
-    const double ur = ((deriv & 3) == 0) ? 1.0 : ((deriv & 3) == 2) ? -1.0 : 0.0;
-    const double ui = ((deriv & 3) == 1) ? 1.0 : ((deriv & 3) == 3) ? -1.0 : 0.0;
-    const double* __restrict__ tw = a.twn;
+    const int M = a.M;
     auto stage_tile = [&](double2* buf, int64_t t) { const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
         stage_rows(reinterpret_cast<double*>(buf), a.in + xt * (2 * P), o, M, a.in_rpb, a.in_blk_stride, inner); };
     const bool in_a = r < 3 * NB, in_b = r < 2 * NA;
-    const int n2 = r % NB, c = r / NB;                       // stage A role
     const int k1 = r % NA, h = r / NA;                       // stage B role
     int64_t t = blockIdx.x;
     int cur = 0;
@@ -209,58 +413,13 @@ k_rbwd_regs(RegArgs a, TileWalk tw_)
         db_cp_wait<1>();
         __syncthreads();
         double2 u[Q];
-        if (in_a) {
-            // Z_k = X1_k + i X2_k (k <= Kmax), Z_{n-k} = conj X1_k + i conj X2_k, X_k = (c_2k + i c_2k+1) / 2, X_0 = c_0
-            auto spec = [&](int k, bool mirrored) -> double2 {
-                if (k > Kmax) return make_double2(0.0, 0.0);
-                const double2 R = in[(2 * k) * P + p];                      // (re line 1, re line 2)
-                if (k == 0) return DERIV ? make_double2(0.0, 0.0) : R;
-                const double2 I = in[(2 * k + 1) * P + p];                  // (im line 1, im line 2)
-                if (DERIV) {
-                    const double ks = a.kscale * k, ks2 = ks * ks;
-                    const double f = 0.5 * ((deriv == 1) ? ks : (deriv == 2) ? ks2 : (deriv == 3) ? ks2 * ks : ks2 * ks2);
-                    const double mr = ur * f, mi = ui * f;
-                    const double2 R2 = make_double2(mr * R.x - mi * I.x, mr * R.y - mi * I.y);
-                    const double2 I2 = make_double2(mi * R.x + mr * I.x, mi * R.y + mr * I.y);
-                    return mirrored ? make_double2(R2.x + I2.y, R2.y - I2.x) : make_double2(R2.x - I2.y, I2.x + R2.y);
-                }
-                return mirrored ? make_double2(0.5 * (R.x + I.y), 0.5 * (R.y - I.x)) : make_double2(0.5 * (R.x - I.y), 0.5 * (I.x + R.y));
-            };
-            double2 lo[Q], hi[Q];
-#pragma unroll
-            for (int b = 0; b < Q; ++b) {
-                lo[b] = spec(NB * b + n2, false);                  // Z[NB b + n2]
-                hi[b] = spec(NB * (Q - b) - n2, true);             // Z[NB (2Q + b) + n2] = mirror of mode n - that
-            }
-            // stage A: size-NA DFT over n1 = Q a + b with the a = 1 third identically zero; this thread's residue c
-            if (c == 0) residue_combine<0, Q, true>(u, lo, hi);
-            else if (c == 1) residue_combine<1, Q, true>(u, lo, hi);
-            else residue_combine<2, Q, true>(u, lo, hi);
-        }
+        if (in_a) rbwd_load_a<Q, NB, DERIV>(in, p, r, M, a.deriv, a.kscale, u);
         __syncthreads();                                           // every input value is consumed: reuse `in` as exchange
-        if (in_a) {
-            DftP2<Q, true>::run(u);
-            double2* dst = in + n2 * P + p;
-#pragma unroll
-            for (int kb = 0; kb < Q; ++kb) {
-                const int kk = 3 * kb + c;                         // output k1
-                dst[kk * NB * P] = cmulc2(u[kb], ldtwn(tw, n2 * kk));
-            }
-        }
+        if (in_a) rbwd_exchange_a<Q, NB>(u, in, a.twn, p, r);
         __syncthreads();
         if (in_b) {
-            // stage B: size-NB DFT over n2 for fixed k1, outputs k2 = 2 m + h; grid index j = k1 + NA k2
-            const double2* src = in + (k1 * NB) * P + p;
             double2 v[H];
-            if (h == 0) {
-#pragma unroll
-                for (int m = 0; m < H; ++m) v[m] = cadd2(src[m * P], src[(m + H) * P]);
-            } else {
-#pragma unroll
-                for (int m = 0; m < H; ++m) v[m] = csub2(src[m * P], src[(m + H) * P]);
-                twiddle_odd_half<true>(v, std::make_integer_sequence<int, H>{});
-            }
-            DftP2<H, true>::run(v);
+            rbwd_stage_b<Q, NB>(in, p, r, v);
             const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
             double* __restrict__ gout = a.out + xt * (2 * P) + 2 * p;
 #pragma unroll
@@ -272,18 +431,6 @@ k_rbwd_regs(RegArgs a, TileWalk tw_)
     db_cp_wait<0>();
 }
 
-// forward stage 2, residue C of the outputs: t[b] = sum_a' W3^(a' C) B[Q a' + b], times W_NA^(b C)
-template <int C, int Q>
-__device__ __forceinline__ void residue_gather(double2 (&u)[Q], const double2* src, int stride)
-{
-#pragma unroll
-    for (int b = 0; b < Q; ++b) {
-        const double2 b0 = src[b * stride], b1 = src[(Q + b) * stride], b2 = src[(2 * Q + b) * stride];
-        u[b] = cadd2(b0, cadd2(mul_tw<C % 3, 3, false>(b1), mul_tw<(2 * C) % 3, 3, false>(b2)));
-    }
-    twiddle_row<C, 3 * Q, false>(u, std::make_integer_sequence<int, Q>{});
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // forward: grid (n rows) -> coefficients (M rows)
 // ---------------------------------------------------------------------------------------------------------
@@ -292,17 +439,12 @@ __global__ void __launch_bounds__(RegGeom<Q, NB>::THREADS, RegGeom<Q, NB>::MINB)
 k_rfwd_regs(RegArgs a, TileWalk tw_)
 {
     using G = RegGeom<Q, NB>;
-    constexpr int NA = G::NA, N = G::N, P = G::P, H = NB / 2;
+    constexpr int N = G::N, P = G::P;
     DB_SMEM(double2, sm);                                   // 2 buffers of [N][P] double2
     const int p = threadIdx.x & (P - 1), r = threadIdx.x >> 3;
     const int64_t inner = a.inner;
-    const int M = a.M, Kmax = (a.M - 1) / 2;
-    const double* __restrict__ tw = a.twn;
     auto stage_tile = [&](double2* buf, int64_t t) { const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
         stage_rows(reinterpret_cast<double*>(buf), a.in + xt * (2 * P), o, N, a.in_rpb, a.in_blk_stride, inner); };
-    const bool in_1 = r < 2 * NA, in_2 = r < 3 * NB;
-    const int j1 = r % NA, h = r / NA;                       // stage 1 role: outputs k2 = 2 m + h of the size-NB DFT
-    const int k2 = r % NB, c = r / NB;                       // stage 2 role: outputs k1 = c + 3 kb of the size-NA DFT
     int64_t t = blockIdx.x;
     int cur = 0;
     if (t < tw_.total) stage_tile(sm, t);
@@ -314,77 +456,140 @@ k_rfwd_regs(RegArgs a, TileWalk tw_)
         db_cp_commit();
         db_cp_wait<1>();
         __syncthreads();
-        double2 v[H];
-        if (in_1) {
-            // stage 1: size-NB DFT over j2 for fixed j1 (grid index j = j1 + NA j2), first radix-2 split (DIF)
-            const double2* src = in + j1 * P + p;
-            if (h == 0) {
-#pragma unroll
-                for (int m = 0; m < H; ++m) v[m] = cadd2(src[(NA * m) * P], src[(NA * (m + H)) * P]);
-            } else {
-#pragma unroll
-                for (int m = 0; m < H; ++m) v[m] = csub2(src[(NA * m) * P], src[(NA * (m + H)) * P]);
-                twiddle_odd_half<false>(v, std::make_integer_sequence<int, H>{});
-            }
-        }
-        __syncthreads();                                           // inputs are consumed: reuse `in` as exchange
-        if (in_1) {
-            DftP2<H, false>::run(v);
-            double2* dst = in + (j1 * NB + h) * P + p;
-#pragma unroll
-            for (int m = 0; m < H; ++m) {
-                const int kk = 2 * m + h;                          // output k2
-                dst[(2 * m) * P] = (kk == 0) ? v[m] : cmul2(v[m], ldtwn(tw, j1 * kk));
-            }
-        }
-        __syncthreads();
-        double2 z[Q];
-        if (in_2) {
-            // stage 2: size-NA DFT over j1 = Q a' + b for fixed k2; this thread's output residue c: k1 = c + 3 kb
-            const double2* src = in + k2 * P + p;
-            if (c == 0) residue_gather<0, Q>(z, src, NB * P);
-            else if (c == 1) residue_gather<1, Q>(z, src, NB * P);
-            else residue_gather<2, Q>(z, src, NB * P);
-            DftP2<Q, false>::run(z);
-        }
-        __syncthreads();
-        if (in_2) {
-            // park the high third (k1 >= 2Q) as Zhi[k1 - 2Q][k2] for the mirror partners
-            double2* dst = in + k2 * P + p;
-#pragma unroll
-            for (int kb = 0; kb < Q; ++kb) {
-                const int kk = 3 * kb + c;
-                if (kk >= 2 * Q) dst[(kk - 2 * Q) * NB * P] = z[kb];
-            }
-        }
-        __syncthreads();
-        if (in_2) {
-            // Z_{n-k} for k = NB k1 + k2 sits at Zhi[(Q - 1 - k1), NB - k2] for k2 > 0, Zhi[Q - k1, 0] for k2 = 0
-            const double sc = 1.0 / N;
+        rfwd_tile<Q, NB>(in, p, r, a, [&] {
             const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
-            double* __restrict__ gout = a.out + xt * (2 * P) + 2 * p;
-            const int k2p = (k2 == 0) ? 0 : NB - k2;
-            const double2* src = in + k2p * P + p;
+            return OutCol{a.out + xt * (2 * P) + 2 * p, o};
+        });
+        __syncthreads();
+    }
+    db_cp_wait<0>();
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Fused x pass of a right-hand side: backward x transforms of the inputs -> quadratic products -> forward x transforms of the
+// outputs, one tile (16 lines x the whole x line) at a time, so that no grid array goes through global memory.
+//
+// A tile walks the host-built schedule `items`:
+//   * held items transform an input that appears in several terms (the velocity components of u.grad(u), u.grad(b)) and keep
+//     this thread's grid values in shared memory (a slot private to the thread, so no barrier guards it);
+//   * term items add coef * a * b (or coef * a) to the output's accumulator, exactly as k_pointwise_pairs does; a term with a
+//     streamed factor first transforms that input (with its x derivative), and its grid values are used straight from registers;
+//   * after the last term of an output the accumulator goes through shared memory into the forward transform, whose coefficient
+//     rows are stored to the output array.
+// Every thread accumulates at the grid points it owns after backward stage B, so products need no exchange.  The coefficient
+// rows of the next transform are in flight (cp.async) from the moment the current ones are in registers (after stage A) until
+// the next item starts: through stage B, the products and, after an output's last term, its forward transform.
+//
+// Shared memory at n = 384, M = 256, three held factors: exchange [N][P] 48 KB + staging [M][P] 32 KB + 3 held tiles 144 KB =
+// 224 KB, one CTA of 384 threads per SM.  Holding a factor in registers instead (32 more per thread, for a second staging slot)
+// takes the kernel past the 168 registers a 384-thread CTA can have and makes it spill.
+// ---------------------------------------------------------------------------------------------------------
+#define XP_STREAM 3             // factor code of the streamed input (0..2: held factors, -1: none)
+
+struct XProdArgs {
+    const double* in;           // stack of level arrays: input s at in + s * in_stride, rows M x inner
+    double* out;                // outputs: o at out + o * out_stride, rows M x inner
+    const double* twn;
+    int64_t inner, in_stride, out_stride;
+    int32_t M;
+    double kscale;
+    const db_xprod_item* items;
+    int32_t n_items;
+    const int32_t* loads;       // src of every item with src >= 0, in item order
+    int32_t n_loads;
+};
+
+template <int Q, int NB> struct XpGeom {
+    static constexpr int N = 3 * Q * NB, THREADS = RegGeom<Q, NB>::THREADS, H = NB / 2;
+    static size_t smem(int M, int n_held)
+    {
+        return sizeof(double2) * ((size_t)N * RR_P + (size_t)M * RR_P + (size_t)n_held * H * THREADS);
+    }
+};
+
+template <int Q, int NB>
+__global__ void __launch_bounds__(RegGeom<Q, NB>::THREADS, 1)
+k_rfft_x_products(XProdArgs a, int64_t total)
+{
+    using G = RegGeom<Q, NB>;
+    constexpr int NA = G::NA, N = G::N, P = G::P, H = NB / 2, THREADS = G::THREADS;
+    DB_SMEM(double2, sm);
+    const int M = a.M;
+    double2* X = sm;                                       // [N][P] exchange / forward staging
+    double2* stg = X + N * P;                              // [M][P] coefficient rows of the next transform
+    double2* hs = stg + M * P;                             // held factors: [H][THREADS] each, private to their thread
+    const int tid = threadIdx.x, p = tid & (P - 1), r = tid >> 3;
+    const bool in_a = r < 3 * NB, in_b = r < 2 * NA;
+    const int k1 = r % NA, h = r / NA;
+    const int64_t inner = a.inner;
+    RegArgs fa;                                            // forward store: plain row addressing into the output arrays
+    fa.in = nullptr; fa.out = a.out; fa.twn = a.twn; fa.inner = inner; fa.M = M; fa.deriv = 0; fa.kscale = 0.0;
+    fa.in_rpb = 0; fa.out_rpb = 0; fa.in_blk_stride = 0; fa.out_blk_stride = 0; fa.out_peers = 0;
+    for (int i = 0; i < 8; ++i) fa.out_blk_ptr[i] = nullptr;
+    // load sequence of this CTA: for each of its tiles, every entry of a.loads
+    int64_t ld_t = blockIdx.x;
+    int ld_k = 0;
+    auto issue = [&] {
+        if (ld_t < total) {
+            stage_rows(reinterpret_cast<double*>(stg), a.in + a.loads[ld_k] * a.in_stride + ld_t * (2 * P), 0, M, 0, 0, inner);
+            if (++ld_k == a.n_loads) { ld_k = 0; ld_t += gridDim.x; }
+        }
+    };
+    issue();
+    db_cp_commit();
+    double2 acc[H];
 #pragma unroll
-            for (int kb = 0; kb < Q; ++kb) {
-                const int kk = 3 * kb + c;                         // k1
-                const int k = NB * kk + k2;
-                if (kk >= Q || k > Kmax) continue;
-                double* row = out_row_ptr(a, gout, o, 2 * k, M, inner);
-                double* row1 = out_row_ptr(a, gout, o, 2 * k + 1, M, inner);
-                const double2 za = z[kb];
-                if (k == 0) {
-                    *reinterpret_cast<double2*>(row) = make_double2(za.x * sc, za.y * sc);
-                    *reinterpret_cast<double2*>(row1) = make_double2(0.0, 0.0);
+    for (int m = 0; m < H; ++m) acc[m] = make_double2(0.0, 0.0);
+    for (int64_t t = blockIdx.x; t < total; t += gridDim.x) {
+        for (int i = 0; i < a.n_items; ++i) {
+            const db_xprod_item* itp = a.items + i;
+            double2 v[H];
+            if (itp->src >= 0) {
+                db_cp_wait<0>();
+                __syncthreads();                           // this input's rows have landed for every thread; X is free
+                double2 u[Q];
+                if (in_a) {
+                    const int deriv = itp->deriv;
+                    if (deriv == 0) rbwd_load_a<Q, NB, false>(stg, p, r, M, 0, a.kscale, u);
+                    else rbwd_load_a<Q, NB, true>(stg, p, r, M, deriv, a.kscale, u);
+                    rbwd_exchange_a<Q, NB>(u, X, a.twn, p, r);
+                }
+                __syncthreads();                           // staging consumed, exchange written
+                issue();
+                db_cp_commit();
+                if (in_b) rbwd_stage_b<Q, NB>(X, p, r, v);
+            }
+            const db_xprod_item it = *itp;                 // (read after the transform: not live across it)
+            if (in_b) {
+                auto factor = [&](int f, int m) -> double2 {
+                    return f == XP_STREAM ? v[m] : hs[(f * H + m) * THREADS + tid];
+                };
+                if (it.flags & DB_XPROD_HELD) {
+#pragma unroll
+                    for (int m = 0; m < H; ++m) hs[(it.a * H + m) * THREADS + tid] = v[m];
                 } else {
-                    const int kbp = (k2 == 0) ? Q - kk : Q - 1 - kk;
-                    const double2 zb = src[kbp * NB * P];
-                    *reinterpret_cast<double2*>(row) = make_double2((za.x + zb.x) * sc, (za.y + zb.y) * sc);
-                    *reinterpret_cast<double2*>(row1) = make_double2((za.y - zb.y) * sc, (zb.x - za.x) * sc);
+#pragma unroll
+                    for (int m = 0; m < H; ++m) {
+                        const double2 va = factor(it.a, m);
+                        const double p0 = it.coef * va.x, p1 = it.coef * va.y;
+                        if (it.b >= 0) {
+                            const double2 vb = factor(it.b, m);
+                            acc[m].x = fma(p0, vb.x, acc[m].x); acc[m].y = fma(p1, vb.y, acc[m].y);
+                        } else { acc[m].x += p0; acc[m].y += p1; }
+                    }
                 }
             }
+            if (it.flags & DB_XPROD_LAST) {
+                __syncthreads();                           // stage B reads of X are done
+                if (in_b) {
+#pragma unroll
+                    for (int m = 0; m < H; ++m) { X[(k1 + NA * (2 * m + h)) * P + p] = acc[m]; acc[m] = make_double2(0.0, 0.0); }
+                }
+                __syncthreads();
+                rfwd_tile<Q, NB>(X, p, r, fa, [&] { return OutCol{a.out + it.out * a.out_stride + t * (2 * P) + 2 * p, 0}; });
+                __syncthreads();
+            }
         }
-        __syncthreads();
     }
     db_cp_wait<0>();
 }
@@ -813,6 +1018,33 @@ int launch_regs(bool fwd, const RegArgs& a, int64_t outer, void* stream)
     return db_check_launch(fwd ? "rfft_forward(regs)" : "rfft_backward(regs)");
 }
 
+template <int Q, int NB>
+int launch_x_products(const XProdArgs& a, int32_t n_held, void* stream)
+{
+    using X = XpGeom<Q, NB>;
+    const size_t bytes = X::smem(a.M, n_held);
+    if (bytes > (size_t)DB_MAX_SMEM) {
+        db_set_error("rfft_x_products: %d held factors at n = %d need %zu bytes of shared memory", (int)n_held, X::N, bytes);
+        return 1;
+    }
+    const int64_t total = a.inner / (2 * RR_P);
+    int per_sm = (int)((size_t)(226 * 1024) / (bytes + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 8) per_sm = 8;
+    int64_t nblk = (int64_t)regs_num_sms() * per_sm;
+    if (nblk > total) nblk = total;
+#ifndef DB_EMU
+    static bool attr = false;
+    if (!attr) {
+        cudaFuncSetAttribute(k_rfft_x_products<Q, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
+        cudaFuncSetAttribute(k_rfft_x_products<Q, NB>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        attr = true;
+    }
+#endif
+    DB_LAUNCH((k_rfft_x_products<Q, NB>), dim3((unsigned)nblk), dim3(X::THREADS), bytes, stream, a, total);
+    return db_check_launch("rfft_x_products");
+}
+
 static long long g_regs_launches = 0;
 }  // namespace
 
@@ -885,5 +1117,38 @@ int db_cheb_regs_try(bool fwd, const db_fft_plan* plan, const double* in, double
         case 48:  return launch_cheb<2, 8>(fwd, a, stream);
         case 24:  return launch_cheb<2, 4>(fwd, a, stream);
         default: --g_regs_launches; return -1;
+    }
+}
+
+// Fused x pass of a quadratic right-hand side (k_rfft_x_products); every case it does not cover is an error: the caller checks
+// coverage first (RealFourierTransform.x_products_supported mirrors these conditions).
+extern "C" int db_rfft_x_products(const db_fft_plan* plan, const double* in, int64_t in_stride, double* out, int64_t out_stride,
+                                  int32_t n_coeff, int64_t inner, double kscale, const db_xprod_item* items, int32_t n_items,
+                                  const int32_t* loads, int32_t n_loads, int32_t n_held, void* stream)
+{
+    const int n = plan->n;
+    const bool ok = plan->half && plan->twn != nullptr && inner >= 2 * RR_P && inner % (2 * RR_P) == 0 && n_coeff % 2 == 0 &&
+                    n_coeff >= 2 && (int64_t)3 * n_coeff <= (int64_t)2 * n && n_held >= 0 && n_held <= 3 && n_items > 0 &&
+                    n_loads > 0 && in_stride % 2 == 0 && out_stride % 2 == 0 &&
+                    ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+    if (!ok) {
+        db_set_error("rfft_x_products: case not covered (n = %d, M = %d, inner = %lld, %d held factors)", n, (int)n_coeff,
+                     (long long)inner, (int)n_held);
+        return 1;
+    }
+    XProdArgs a;
+    a.in = in; a.out = out; a.twn = plan->twn; a.inner = inner; a.in_stride = in_stride; a.out_stride = out_stride;
+    a.M = n_coeff; a.kscale = kscale; a.items = items; a.n_items = n_items; a.loads = loads; a.n_loads = n_loads;
+    ++g_regs_launches;
+    switch (n) {
+        case 384: return launch_x_products<8, 16>(a, n_held, stream);
+        case 192: return launch_x_products<4, 16>(a, n_held, stream);
+        case 96:  return launch_x_products<4, 8>(a, n_held, stream);
+        case 48:  return launch_x_products<2, 8>(a, n_held, stream);
+        case 24:  return launch_x_products<2, 4>(a, n_held, stream);
+        default:
+            --g_regs_launches;
+            db_set_error("rfft_x_products: no kernel for n = %d", n);
+            return 1;
     }
 }

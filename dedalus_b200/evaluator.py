@@ -269,9 +269,11 @@ class RHSPlan:
         # ---- backward prefix tree: level order = axes from last to first
         self.axes_order = list(range(dim - 1, -1, -1))
         self._build_tree()
-        # ---- buffers
-        self.grid_in = torch.empty((self.n_in,) + self.gshape, dtype=torch.float64, device=dev)
-        self.grid_out = torch.empty((self.n_out,) + self.gshape, dtype=torch.float64, device=dev)
+        # ---- grid buffers of the separate passes (allocated on first use: the fused x pass does not need them)
+        self._grid_in = self._grid_out = None
+        # ---- fused x pass (backward x transforms + products + forward x transforms in one kernel), or None
+        self.xprod = self._build_x_products()
+        self.use_x_products = self.xprod is not None
         # ---- output destinations in the equation arena and forward plans
         self.out_dest = []
         for ie, comp, tl in outputs:
@@ -279,6 +281,87 @@ class RHSPlan:
             tsh, shp = arena.shapes[ie]
             off = arena.offsets[ie] + comp * int(np.prod(shp))
             self.out_dest.append((off, shp, eq['bases']))
+
+    @property
+    def grid_in(self):
+        if self._grid_in is None:
+            import torch
+            self._grid_in = torch.empty((self.n_in,) + self.gshape, dtype=torch.float64, device=self.device)
+        return self._grid_in
+
+    @property
+    def grid_out(self):
+        if self._grid_out is None:
+            import torch
+            self._grid_out = torch.empty((self.n_out,) + self.gshape, dtype=torch.float64, device=self.device)
+        return self._grid_out
+
+    def _build_x_products(self):
+        """Schedule of the fused x pass (csrc/rfft_regs.cu k_rfft_x_products), or None where the separate passes stay.
+
+        The x axis is the last backward and the first forward pass, so a tile of 16 adjacent lines holds everything the products
+        need once its lines are transformed along x: the inputs' level-(dim-2) coefficient arrays are read once and the outputs'
+        x coefficients written once, with no grid array in global memory.  Inputs that appear in more than one term (the velocity
+        components of u.grad(u), u.grad(b)) are held on chip for the whole tile; every other input is transformed right before
+        its one term.  DB_RHS_FUSED=0 keeps the separate passes (for A/B timing)."""
+        import os, torch
+        from collections import Counter
+        from .transforms import cached_plan, RealFourierTransform
+        dim = self.dist.dim
+        if os.environ.get("DB_RHS_FUSED", "1") == "0" or os.environ.get("DB_FFT_REGS", "1") == "0":
+            return None
+        if self.P != 1 or dim < 2 or self.grid_leaves or self.broadcast_leaves or self.pairs is None:
+            return None
+        px = cached_plan(self.bases[0], self.dealias[0])
+        if not isinstance(px, RealFourierTransform):
+            return None
+        final, parents = self.levels[dim - 1], self.levels[dim - 2]
+        src, deriv = [], []
+        for key in self.leaf_of_input:
+            nd = final[key]
+            p = cached_plan(nd['field'].bases[0], self.dealias[0])
+            if not isinstance(p, RealFourierTransform) or (p.N, p.M, p.kscale) != (px.N, px.M, px.kscale):
+                return None
+            src.append(parents[nd['parent']]['index']); deriv.append(nd['deriv'])
+        terms = [(o, coef, idxs) for o, (ie, comp, tl) in enumerate(self.outputs) for coef, idxs in tl]
+        count = Counter(i for _, _, idxs in terms for i in idxs)
+        held = {}
+        for _, _, idxs in terms:
+            for i in idxs:
+                if count[i] > 1 and i not in held:
+                    held[i] = len(held)
+            if len(idxs) == 2 and all(count[i] == 1 for i in idxs):
+                held[idxs[0]] = len(held)             # a product of two single-use inputs: hold the first, stream the second
+        inner = int(np.prod(self.gshape[1:], dtype=np.int64))
+        if not px.x_products_supported(inner, len(held)):
+            return None
+        rec = []                                      # db_xprod_item: coef, src, deriv, a, b, out, flags
+        for i, slot in held.items():
+            rec.append((0.0, src[i], deriv[i], slot, -1, -1, 1))                                   # DB_XPROD_HELD
+        for k, (o, coef, idxs) in enumerate(terms):
+            streamed = [i for i in idxs if i not in held]
+            code = [held.get(i, 3) for i in idxs] + [-1]                                          # 3: the streamed input
+            last = k + 1 == len(terms) or terms[k + 1][0] != o
+            rec.append((coef, src[streamed[0]] if streamed else -1, deriv[streamed[0]] if streamed else 0,
+                        code[0], code[1], o, 2 if last else 0))                                    # DB_XPROD_LAST
+        items = np.array(rec, dtype=np.dtype([('coef', '<f8'), ('src', '<i4'), ('deriv', '<i4'), ('a', '<i4'), ('b', '<i4'),
+                                              ('out', '<i4'), ('flags', '<i4')]))
+        loads = items['src'][items['src'] >= 0]
+        if len(loads) == 0:
+            return None
+        return dict(plan=px, inner=inner, n_held=len(held), n_items=len(items),
+                    items=torch.from_numpy(np.frombuffer(items.tobytes(), dtype=np.uint8).copy()).to(self.device),
+                    loads=torch.from_numpy(loads.astype(np.int32)).to(self.device))
+
+    def _x_products(self, cin):
+        """Fused x pass from the level-(dim-2) stack into the x-forward scratch that the next forward pass reads."""
+        from .solvers import Timed
+        xp = self.xprod
+        px, inner = xp['plan'], xp['inner']
+        out = self._scratch(('fwd', 0), (self.n_out, px.M) + tuple(self.gshape[1:]))
+        with Timed(self.solver.prof, "rhs_x_products", 8 * (self.n_in + self.n_out) * px.M * inner):
+            px.x_products(cin, out, inner, xp['items'], xp['n_items'], xp['loads'], xp['n_held'])
+        return out
 
     # ------------------------------------------------------------------------------------------------
     def _add_constant(self, ie, eq, value, comp=0):
@@ -381,10 +464,13 @@ class RHSPlan:
         for f in in_tree.values():
             if f.layout != 'c':
                 f.change_layout('c')          # non-state fields (forcings, NCCs) may have been set on the grid
+        fused = self.use_x_products and not grid_only
         bufs = [None] * dim
         for lvl, ax in enumerate(self.axes_order if in_tree else []):
             nodes = self.levels[lvl]
             final = (lvl == dim - 1)
+            if final and fused:
+                break
             prev = bufs[lvl - 1] if lvl > 0 else None
             if self.P > 1 and dim >= 3 and lvl == dim - 2 and self._blocked_bwd_ok():
                 # the y pass writes the all-to-all send buffer directly and the x pass reads the receive buffer directly
@@ -416,20 +502,16 @@ class RHSPlan:
                     dst = bufs[lvl][nd['index']]
                 with Timed(self.solver.prof, f"transform_bwd_axis{ax}", 8 * (src.numel() + dst.numel())):
                     plan.backward(src, dst, ax, deriv=nd['deriv'])
-        # ---- phase 2: pointwise products
-        with Timed(self.solver.prof, "pointwise", 8 * self.npoints * (self.n_in + self.n_out)):
-          if self.pairs is not None and self.grid_in.data_ptr() % 16 == 0 and self.grid_out.data_ptr() % 16 == 0:
-              get_lib().call("db_pointwise_pairs", _dptr(self.grid_in), _dptr(self.grid_out), self.npoints, self.n_in, self.n_out,
-                             _dptr(self.term_ptr), _dptr(self.pairs), _stream())
-          else:
-              get_lib().call("db_pointwise", _dptr(self.grid_in), _dptr(self.grid_out), self.npoints, self.n_in, self.n_out,
-                             _dptr(self.term_ptr), _dptr(self.coef), _dptr(self.fac_ptr), _dptr(self.fac), self.nfac, _stream())
+        if fused:
+            # ---- phases 2 and the x pass of phase 3 in one kernel
+            cur = self._x_products(bufs[dim - 2])
+        else:
+            cur = self._products()
         if grid_only:
-            return self.grid_out
+            return cur
         # ---- phase 3: forward transforms (axes first -> last), all outputs stacked
-        cur = self.grid_out
         blocked_fwd = self.P > 1 and dim >= 3 and self._blocked_fwd_ok()
-        for ax in range(dim):
+        for ax in range(1 if fused else 0, dim):
             basis = self.bases[ax]
             if blocked_fwd and ax == 0:
                 cur = self._forward_blocked_xy(cur)
@@ -464,6 +546,20 @@ class RHSPlan:
                     dst = eq_arena_tensor[off:off + n].view(shp)
                     with Timed(self.solver.prof, f"transform_fwd_axis{ax}", 8 * (cur[o].numel() + dst.numel())):
                         plan.forward(cur[o], dst, ax)
+
+    def _products(self):
+        """Phase 2 of the separate passes: products of the backward-transformed inputs on the grid into grid_out."""
+        from .transforms import _dptr, _stream
+        from .lib import get_lib
+        from .solvers import Timed
+        with Timed(self.solver.prof, "pointwise", 8 * self.npoints * (self.n_in + self.n_out)):
+          if self.pairs is not None and self.grid_in.data_ptr() % 16 == 0 and self.grid_out.data_ptr() % 16 == 0:
+              get_lib().call("db_pointwise_pairs", _dptr(self.grid_in), _dptr(self.grid_out), self.npoints, self.n_in, self.n_out,
+                             _dptr(self.term_ptr), _dptr(self.pairs), _stream())
+          else:
+              get_lib().call("db_pointwise", _dptr(self.grid_in), _dptr(self.grid_out), self.npoints, self.n_in, self.n_out,
+                             _dptr(self.term_ptr), _dptr(self.coef), _dptr(self.fac_ptr), _dptr(self.fac), self.nfac, _stream())
+        return self.grid_out
 
     def _fwd_plan_last(self, prod_basis, target_basis):
         from .transforms import FastChebyshevTransform, cached_plan

@@ -131,6 +131,27 @@ class RealFourierTransform:
         if not ok:
             raise RuntimeError("peer real-Fourier transform not covered (blocked_supported() out of sync with the kernels)")
 
+    # ---- the x pass of a quadratic right-hand side fused with its products (include/dedalus_b200.h db_rfft_x_products)
+    _XP_GEOM = {24: (2, 4), 48: (2, 8), 96: (4, 8), 192: (4, 16), 384: (8, 16)}       # n -> (Q, NB) of csrc/rfft_regs.cu
+
+    def x_products_supported(self, inner, n_held):
+        """Mirror of the coverage test of db_rfft_x_products and its shared-memory budget (XpGeom::smem)."""
+        if self.N not in self._XP_GEOM or not (self.M % 2 == 0 and self.M >= 2 and 3 * self.M <= 2 * self.N):
+            return False
+        if inner < 16 or inner % 16 != 0 or not 0 <= n_held <= 3:
+            return False
+        q, nb = self._XP_GEOM[self.N]
+        threads = max(3 * nb * 8, 6 * q * 8)
+        smem = 16 * (self.N * 8 + self.M * 8 + n_held * (nb // 2) * threads)
+        return smem <= 227 * 1024
+
+    def x_products(self, cin, cout, inner, items, n_items, loads, n_held):
+        """cin: (n_src, M, ...) coefficient stack; cout: (n_out, M, ...) coefficients of the outputs; items / loads: the device schedule."""
+        _check(cin, "cin"); _check(cout, "cout")
+        plan = DevicePlan(self.N, 'real', cin.device)
+        get_lib().call("db_rfft_x_products", plan.ref(), _dptr(cin), self.M * inner, _dptr(cout), self.M * inner, self.M, inner,
+                       float(self.kscale), _dptr(items), n_items, _dptr(loads), int(loads.numel()), n_held, _stream())
+
     def forward_blocked(self, g_ptr, c_ptr, outer, inner, device, in_block=(0, 0), out_block=(0, 0)):
         plan = DevicePlan(self.N, 'real', device)
         ok = get_lib().call_optional("db_rfft_forward_blocked", plan.ref(), C.c_void_p(g_ptr), C.c_void_p(c_ptr), outer, self.M, inner,

@@ -153,6 +153,20 @@ int db_pointwise(const double* in, double* out, int64_t npoints, int32_t n_in, i
 typedef struct { double coef; int32_t a; int32_t b; } db_pair_term;
 int db_pointwise_pairs(const double* in, double* out, int64_t npoints, int32_t n_in, int32_t n_out,
                        const int32_t* term_ptr, const db_pair_term* terms, void* stream);
+/* The x pass of a quadratic right-hand side fused with its products (real Fourier x axis, n in 24, 48, 96, 192, 384):
+ * backward x transforms of the inputs, the products, and the forward x transforms of the outputs, one tile of 16 lines at a time,
+ * with no grid array in global memory.  in: stack of (n_coeff, inner) coefficient arrays, input s at in + s * in_stride;
+ * out: output o at out + o * out_stride, (n_coeff, inner).  The schedule (device arrays) is walked once per tile:
+ *   item with DB_XPROD_HELD: transform input `src` with x derivative `deriv` and keep its grid values as held factor `a` (0..2);
+ *   other items: one term coef * a * b (b < 0: coef * a) of output `out`, factors coded 0..2 = held, 3 = input `src` transformed
+ *   just before (src < 0: no transform), accumulated exactly as db_pointwise_pairs does; DB_XPROD_LAST after an output's last term.
+ * loads: the src of every item with src >= 0, in item order.  inner % 16 == 0, arrays 16-byte aligned, n_held <= 3. */
+typedef struct { double coef; int32_t src; int32_t deriv; int32_t a; int32_t b; int32_t out; int32_t flags; } db_xprod_item;
+#define DB_XPROD_HELD 1
+#define DB_XPROD_LAST 2
+int db_rfft_x_products(const db_fft_plan* plan, const double* in, int64_t in_stride, double* out, int64_t out_stride,
+                       int32_t n_coeff, int64_t inner, double kscale, const db_xprod_item* items, int32_t n_items,
+                       const int32_t* loads, int32_t n_loads, int32_t n_held, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Pencil systems (S1-S4).  A batch holds S structurally identical systems of size n; one thread owns one system.
