@@ -10,7 +10,7 @@
 //   * dealias padding is structural: coefficient modes k >= n/3 are zero, which is exactly the middle third of the
 //     first radix-3 split of stage A (backward) / the discarded third of its outputs (forward), so that third of the
 //     butterflies is never computed and the padded zeros / truncated modes are never touched in memory.
-// One CTA = 16 lines (8 complex pairs, 128-byte rows) x the whole line; 48 KB of shared memory.
+// One CTA = 16 lines (8 complex pairs, 128-byte rows) x the whole line; 48 KB of shared memory (tile height P below).
 // Conventions as in fft.cu (reference core/transforms.py:469-509, 537-565): cos / -sin interleaved coefficients,
 // forward scaled by 2/n (1/n for k = 0), sin(0) slot zero, Nyquist dropped.
 #include "db_common.cuh"
@@ -127,23 +127,27 @@ __device__ __forceinline__ double2 ldtwn(const double* __restrict__ tw, int j) {
 __device__ __forceinline__ double2 cmulc2(double2 a, double2 w) { return make_double2(a.x * w.x + a.y * w.y, a.y * w.x - a.x * w.y); }
 __device__ __forceinline__ double2 cmul2(double2 a, double2 w) { return make_double2(a.x * w.x - a.y * w.y, a.x * w.y + a.y * w.x); }
 
-#define RR_P 8          // complex line pairs per CTA tile (16 real lines)
+// Tile height: P complex line pairs (2P real lines) per CTA tile, P = 8 or 4.  The per-pair arithmetic does not depend on P,
+// so both tile heights give bitwise-equal results; smaller tiles mean smaller CTAs, more of them per SM in different phases.
+// Both divide the 16 lines the coverage tests below require of `inner`.
+#define RR_LINES 16
 
-// Persistent CTAs walk the tiles (tile = 16 adjacent lines x the whole line length) with the NEXT tile's input rows in
+// Persistent CTAs walk the tiles (tile = 2P adjacent lines x the whole line length) with the NEXT tile's input rows in
 // flight (16-byte cp.async, L1-bypassing) while the current tile is transformed: two shared-memory buffers of
-// n x 128 bytes; the stage A -> stage B exchange reuses the buffer the current tile's input was staged in.
+// n x 16P bytes; the stage A -> stage B exchange reuses the buffer the current tile's input was staged in.
 struct TileWalk {
     int64_t tiles_per_outer, total;
 };
 
-// stage `rows` rows of 16 doubles (row stride `inner`) into buf[row][16]
+// stage `rows` rows of 2P doubles (row stride `inner`) into buf[row][2P]
+template <int P>
 __device__ __forceinline__ void stage_rows(double* buf, const double* __restrict__ src, int64_t o, int rows, int rpb,
                                            int64_t blk_stride, int64_t inner)
 {
     // src already points at the tile's first column; row r of outer index o is at row_offset(...)
-    for (int idx = threadIdx.x; idx < rows * 8; idx += blockDim.x) {
-        const int row = idx >> 3, seg = idx & 7;
-        db_cp_async16(buf + row * 16 + seg * 2, src + row_offset(o, row, rows, rpb, blk_stride, inner) + seg * 2);
+    for (int idx = threadIdx.x; idx < rows * P; idx += blockDim.x) {
+        const int row = (unsigned)idx / P, seg = (unsigned)idx % P;
+        db_cp_async16(buf + row * (2 * P) + seg * 2, src + row_offset(o, row, rows, rpb, blk_stride, inner) + seg * 2);
     }
 }
 
@@ -151,12 +155,21 @@ __device__ __forceinline__ void stage_rows(double* buf, const double* __restrict
 //   stage A (size NA = 3Q): thread (c, n2, p) computes the Q outputs k1 = c + 3 kb of the radix-3 residue c
 //   stage B (size NB):      thread (h, k1, p) computes the NB/2 outputs k2 = 2 m + h (first radix-2 split, DIF)
 // (forward: the same two splits in the opposite order).  3 NB P threads work in stage A and 6 Q P in stage B: 384 = 384
-// at n = 384, at ~80 registers, so two CTAs (24 warps) are resident per SM and every warp works in both stages.
-template <int Q, int NB> struct RegGeom {
-    static constexpr int NA = 3 * Q, N = NA * NB, P = RR_P;
+// at n = 384 and P = 8, at ~80 registers, so two CTAs (24 warps) are resident per SM and every warp works in both stages.
+// minb() keeps 768 threads per SM at every P (the same register budget per thread) where shared memory allows.  The forward and
+// the derivative backward transforms of lines of 192 or more points need more than the ~80 registers that leaves: they spill
+// (320 and 460 bytes at n = 384) and run at about half the bandwidth of the plain backward.  minb(true) gives them the whole
+// register file of one CTA (no spills in the forward, 88 bytes in the backward), which is faster despite the single CTA per SM;
+// the launches size their grids from the resulting occupancy.
+template <int Q, int NB, int P> struct RegGeom {
+    static constexpr int NA = 3 * Q, N = NA * NB;
     static constexpr int TA = 3 * NB * P, TB = 6 * Q * P;
     static constexpr int THREADS = TA > TB ? TA : TB;
-    static constexpr int MINB = (2 * N * P * 16 + 1024) * 2 <= 226 * 1024 ? 2 : 1;
+    static constexpr int minb(bool full_regs = false)
+    {
+        const int fit = (int)((226 * 1024) / (2 * N * P * 16 + 1024));
+        return full_regs && N >= 192 ? 1 : fit < 1 ? 1 : (fit < 16 / P ? fit : 16 / P);
+    }
 };
 
 template <bool INV, int N, int... M>
@@ -184,10 +197,9 @@ __device__ __forceinline__ void residue_gather(double2 (&u)[Q], const double2* s
 
 // backward, load + stage A: spectrum of the staged coefficient rows `in` ([M][P] double2: row 2k = re, 2k+1 = im of mode k
 // for both lines of every pair) with (i k kscale)^deriv applied, then this thread's residue of the size-NA DFT (threads r < 3 NB)
-template <int Q, int NB, bool DERIV>
+template <int Q, int NB, int P, bool DERIV>
 __device__ __forceinline__ void rbwd_load_a(const double2* in, int p, int r, int M, int deriv_, double kscale, double2 (&u)[Q])
 {
-    constexpr int P = RR_P;
     const int Kmax = (M - 1) / 2;
     const int deriv = DERIV ? deriv_ : 0;
     // (i k kscale)^deriv = (ur + i ui) (k kscale)^deriv
@@ -231,10 +243,9 @@ __device__ __forceinline__ void rbwd_load_a(const double2* in, int p, int r, int
 }
 
 // backward, end of stage A: radix-2 part and twiddle, stored to the exchange buffer ([N][P] double2, threads r < 3 NB)
-template <int Q, int NB>
+template <int Q, int NB, int P>
 __device__ __forceinline__ void rbwd_exchange_a(double2 (&u)[Q], double2* xch, const double* __restrict__ tw, int p, int r)
 {
-    constexpr int P = RR_P;
     const int n2 = r % NB, c = r / NB;
     DftP2<Q, true>::run(u);
     double2* dst = xch + n2 * P + p;
@@ -247,10 +258,10 @@ __device__ __forceinline__ void rbwd_exchange_a(double2 (&u)[Q], double2* xch, c
 
 // backward stage B (threads r < 6 Q): size-NB DFT over n2 for fixed k1 = r % NA, outputs k2 = 2 m + h (h = r / NA), so v[m] is
 // the pair's grid value at j = k1 + NA (2 m + h)
-template <int Q, int NB>
+template <int Q, int NB, int P>
 __device__ __forceinline__ void rbwd_stage_b(const double2* xch, int p, int r, double2 (&v)[NB / 2])
 {
-    constexpr int P = RR_P, NA = 3 * Q, H = NB / 2;
+    constexpr int NA = 3 * Q, H = NB / 2;
     const int k1 = r % NA, h = r / NA;
     const double2* src = xch + (k1 * NB) * P + p;
     if (h == 0) {
@@ -266,10 +277,10 @@ __device__ __forceinline__ void rbwd_stage_b(const double2* xch, int p, int r, d
 
 // forward stage 1 load (threads r < 6 Q): first radix-2 split (DIF) of the size-NB DFT over j2 for fixed j1 = r % NA of the staged
 // grid rows `in` ([N][P] double2, grid index j = j1 + NA j2)
-template <int Q, int NB>
+template <int Q, int NB, int P>
 __device__ __forceinline__ void rfwd_load_1(const double2* in, int p, int r, double2 (&v)[NB / 2])
 {
-    constexpr int P = RR_P, NA = 3 * Q, H = NB / 2;
+    constexpr int NA = 3 * Q, H = NB / 2;
     const int j1 = r % NA, h = r / NA;
     const double2* src = in + j1 * P + p;
     if (h == 0) {
@@ -283,10 +294,10 @@ __device__ __forceinline__ void rfwd_load_1(const double2* in, int p, int r, dou
 }
 
 // forward, end of stage 1: the rest of the size-NB DFT and the twiddle, stored to the exchange buffer
-template <int Q, int NB>
+template <int Q, int NB, int P>
 __device__ __forceinline__ void rfwd_exchange_1(double2 (&v)[NB / 2], double2* xch, const double* __restrict__ tw, int p, int r)
 {
-    constexpr int P = RR_P, NA = 3 * Q, H = NB / 2;
+    constexpr int NA = 3 * Q, H = NB / 2;
     const int j1 = r % NA, h = r / NA;
     DftP2<H, false>::run(v);
     double2* dst = xch + (j1 * NB + h) * P + p;
@@ -299,10 +310,9 @@ __device__ __forceinline__ void rfwd_exchange_1(double2 (&v)[NB / 2], double2* x
 
 // forward stage 2 (threads r < 3 NB): size-NA DFT over j1 = Q a' + b for fixed k2 = r % NB; this thread's output residue
 // c = r / NB: z[kb] is mode k1 = c + 3 kb
-template <int Q, int NB>
+template <int Q, int NB, int P>
 __device__ __forceinline__ void rfwd_stage_2(const double2* xch, int p, int r, double2 (&z)[Q])
 {
-    constexpr int P = RR_P;
     const int k2 = r % NB, c = r / NB;
     const double2* src = xch + k2 * P + p;
     if (c == 0) residue_gather<0, Q>(z, src, NB * P);
@@ -312,10 +322,9 @@ __device__ __forceinline__ void rfwd_stage_2(const double2* xch, int p, int r, d
 }
 
 // forward: park the high third (k1 >= 2Q) as Zhi[k1 - 2Q][k2] for the mirror partners
-template <int Q, int NB>
+template <int Q, int NB, int P>
 __device__ __forceinline__ void rfwd_park(const double2 (&z)[Q], double2* xch, int p, int r)
 {
-    constexpr int P = RR_P;
     const int k2 = r % NB, c = r / NB;
     double2* dst = xch + k2 * P + p;
 #pragma unroll
@@ -326,11 +335,11 @@ __device__ __forceinline__ void rfwd_park(const double2 (&z)[Q], double2* xch, i
 }
 
 // forward: the two real lines' cos / -sin coefficients of every mode k <= Kmax this thread owns, scaled, stored to rows 2k, 2k+1
-template <int Q, int NB>
+template <int Q, int NB, int P>
 __device__ __forceinline__ void rfwd_store(const double2 (&z)[Q], const double2* xch, int p, int r, const RegArgs& a, double* gout,
                                            int64_t o)
 {
-    constexpr int P = RR_P, N = 3 * Q * NB;
+    constexpr int N = 3 * Q * NB;
     const int k2 = r % NB, c = r / NB;
     const int M = a.M, Kmax = (a.M - 1) / 2;
     const int64_t inner = a.inner;
@@ -363,42 +372,42 @@ struct OutCol { double* g; int64_t o; };       // a pair's column in the output 
 // the whole forward transform of the grid tile staged in `buf` ([N][P] double2), which is also its exchange buffer; every
 // thread of the CTA calls it (it contains barriers), and `buf` may be overwritten once the caller has passed a barrier after it.
 // dest() -> (this pair's column in the output rows, outer index) is evaluated only at the store.
-template <int Q, int NB, class Dest>
+template <int Q, int NB, int P, class Dest>
 __device__ __forceinline__ void rfwd_tile(double2* buf, int p, int r, const RegArgs& a, Dest dest)
 {
     constexpr int NA = 3 * Q, H = NB / 2;
     const bool in_1 = r < 2 * NA, in_2 = r < 3 * NB;
     double2 v[H];
-    if (in_1) rfwd_load_1<Q, NB>(buf, p, r, v);
+    if (in_1) rfwd_load_1<Q, NB, P>(buf, p, r, v);
     __syncthreads();                                           // inputs are consumed: reuse `buf` as exchange
-    if (in_1) rfwd_exchange_1<Q, NB>(v, buf, a.twn, p, r);
+    if (in_1) rfwd_exchange_1<Q, NB, P>(v, buf, a.twn, p, r);
     __syncthreads();
     double2 z[Q];
-    if (in_2) rfwd_stage_2<Q, NB>(buf, p, r, z);
+    if (in_2) rfwd_stage_2<Q, NB, P>(buf, p, r, z);
     __syncthreads();
-    if (in_2) rfwd_park<Q, NB>(z, buf, p, r);
+    if (in_2) rfwd_park<Q, NB, P>(z, buf, p, r);
     __syncthreads();
     if (in_2) {
         const auto d = dest();
-        rfwd_store<Q, NB>(z, buf, p, r, a, d.g, d.o);
+        rfwd_store<Q, NB, P>(z, buf, p, r, a, d.g, d.o);
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------
 // backward: coefficients (M rows) -> grid (n rows)
 // ---------------------------------------------------------------------------------------------------------
-template <int Q, int NB, bool DERIV>
-__global__ void __launch_bounds__(RegGeom<Q, NB>::THREADS, RegGeom<Q, NB>::MINB)
+template <int Q, int NB, int P, bool DERIV>
+__global__ void __launch_bounds__((RegGeom<Q, NB, P>::THREADS), (RegGeom<Q, NB, P>::minb(DERIV)))
 k_rbwd_regs(RegArgs a, TileWalk tw_)
 {
-    using G = RegGeom<Q, NB>;
-    constexpr int NA = G::NA, N = G::N, P = G::P, H = NB / 2;
+    using G = RegGeom<Q, NB, P>;
+    constexpr int NA = G::NA, N = G::N, H = NB / 2;
     DB_SMEM(double2, sm);                                   // 2 buffers of [N][P] double2
-    const int p = threadIdx.x & (P - 1), r = threadIdx.x >> 3;
+    const int p = threadIdx.x % P, r = threadIdx.x / P;
     const int64_t inner = a.inner;
     const int M = a.M;
     auto stage_tile = [&](double2* buf, int64_t t) { const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
-        stage_rows(reinterpret_cast<double*>(buf), a.in + xt * (2 * P), o, M, a.in_rpb, a.in_blk_stride, inner); };
+        stage_rows<P>(reinterpret_cast<double*>(buf), a.in + xt * (2 * P), o, M, a.in_rpb, a.in_blk_stride, inner); };
     const bool in_a = r < 3 * NB, in_b = r < 2 * NA;
     const int k1 = r % NA, h = r / NA;                       // stage B role
     int64_t t = blockIdx.x;
@@ -413,13 +422,13 @@ k_rbwd_regs(RegArgs a, TileWalk tw_)
         db_cp_wait<1>();
         __syncthreads();
         double2 u[Q];
-        if (in_a) rbwd_load_a<Q, NB, DERIV>(in, p, r, M, a.deriv, a.kscale, u);
+        if (in_a) rbwd_load_a<Q, NB, P, DERIV>(in, p, r, M, a.deriv, a.kscale, u);
         __syncthreads();                                           // every input value is consumed: reuse `in` as exchange
-        if (in_a) rbwd_exchange_a<Q, NB>(u, in, a.twn, p, r);
+        if (in_a) rbwd_exchange_a<Q, NB, P>(u, in, a.twn, p, r);
         __syncthreads();
         if (in_b) {
             double2 v[H];
-            rbwd_stage_b<Q, NB>(in, p, r, v);
+            rbwd_stage_b<Q, NB, P>(in, p, r, v);
             const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
             double* __restrict__ gout = a.out + xt * (2 * P) + 2 * p;
 #pragma unroll
@@ -434,17 +443,17 @@ k_rbwd_regs(RegArgs a, TileWalk tw_)
 // ---------------------------------------------------------------------------------------------------------
 // forward: grid (n rows) -> coefficients (M rows)
 // ---------------------------------------------------------------------------------------------------------
-template <int Q, int NB>
-__global__ void __launch_bounds__(RegGeom<Q, NB>::THREADS, RegGeom<Q, NB>::MINB)
+template <int Q, int NB, int P>
+__global__ void __launch_bounds__((RegGeom<Q, NB, P>::THREADS), (RegGeom<Q, NB, P>::minb(true)))
 k_rfwd_regs(RegArgs a, TileWalk tw_)
 {
-    using G = RegGeom<Q, NB>;
-    constexpr int N = G::N, P = G::P;
+    using G = RegGeom<Q, NB, P>;
+    constexpr int N = G::N;
     DB_SMEM(double2, sm);                                   // 2 buffers of [N][P] double2
-    const int p = threadIdx.x & (P - 1), r = threadIdx.x >> 3;
+    const int p = threadIdx.x % P, r = threadIdx.x / P;
     const int64_t inner = a.inner;
     auto stage_tile = [&](double2* buf, int64_t t) { const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
-        stage_rows(reinterpret_cast<double*>(buf), a.in + xt * (2 * P), o, N, a.in_rpb, a.in_blk_stride, inner); };
+        stage_rows<P>(reinterpret_cast<double*>(buf), a.in + xt * (2 * P), o, N, a.in_rpb, a.in_blk_stride, inner); };
     int64_t t = blockIdx.x;
     int cur = 0;
     if (t < tw_.total) stage_tile(sm, t);
@@ -456,7 +465,7 @@ k_rfwd_regs(RegArgs a, TileWalk tw_)
         db_cp_commit();
         db_cp_wait<1>();
         __syncthreads();
-        rfwd_tile<Q, NB>(in, p, r, a, [&] {
+        rfwd_tile<Q, NB, P>(in, p, r, a, [&] {
             const int64_t o = t / tw_.tiles_per_outer, xt = t - o * tw_.tiles_per_outer;
             return OutCol{a.out + xt * (2 * P) + 2 * p, o};
         });
@@ -499,26 +508,27 @@ struct XProdArgs {
     int32_t n_loads;
 };
 
-template <int Q, int NB> struct XpGeom {
-    static constexpr int N = 3 * Q * NB, THREADS = RegGeom<Q, NB>::THREADS, H = NB / 2;
+// MINB: the register budget per thread (168 at n = 384) is the same at every tile height: 8 / P CTAs of 48 P threads per SM
+template <int Q, int NB, int P> struct XpGeom {
+    static constexpr int N = 3 * Q * NB, THREADS = RegGeom<Q, NB, P>::THREADS, H = NB / 2, MINB = 8 / P;
     static size_t smem(int M, int n_held)
     {
-        return sizeof(double2) * ((size_t)N * RR_P + (size_t)M * RR_P + (size_t)n_held * H * THREADS);
+        return sizeof(double2) * ((size_t)N * P + (size_t)M * P + (size_t)n_held * H * THREADS);
     }
 };
 
-template <int Q, int NB>
-__global__ void __launch_bounds__(RegGeom<Q, NB>::THREADS, 1)
+template <int Q, int NB, int P>
+__global__ void __launch_bounds__((XpGeom<Q, NB, P>::THREADS), (XpGeom<Q, NB, P>::MINB))
 k_rfft_x_products(XProdArgs a, int64_t total)
 {
-    using G = RegGeom<Q, NB>;
-    constexpr int NA = G::NA, N = G::N, P = G::P, H = NB / 2, THREADS = G::THREADS;
+    using G = RegGeom<Q, NB, P>;
+    constexpr int NA = G::NA, N = G::N, H = NB / 2, THREADS = G::THREADS;
     DB_SMEM(double2, sm);
     const int M = a.M;
     double2* X = sm;                                       // [N][P] exchange / forward staging
     double2* stg = X + N * P;                              // [M][P] coefficient rows of the next transform
     double2* hs = stg + M * P;                             // held factors: [H][THREADS] each, private to their thread
-    const int tid = threadIdx.x, p = tid & (P - 1), r = tid >> 3;
+    const int tid = threadIdx.x, p = threadIdx.x % P, r = threadIdx.x / P;
     const bool in_a = r < 3 * NB, in_b = r < 2 * NA;
     const int k1 = r % NA, h = r / NA;
     const int64_t inner = a.inner;
@@ -531,7 +541,7 @@ k_rfft_x_products(XProdArgs a, int64_t total)
     int ld_k = 0;
     auto issue = [&] {
         if (ld_t < total) {
-            stage_rows(reinterpret_cast<double*>(stg), a.in + a.loads[ld_k] * a.in_stride + ld_t * (2 * P), 0, M, 0, 0, inner);
+            stage_rows<P>(reinterpret_cast<double*>(stg), a.in + a.loads[ld_k] * a.in_stride + ld_t * (2 * P), 0, M, 0, 0, inner);
             if (++ld_k == a.n_loads) { ld_k = 0; ld_t += gridDim.x; }
         }
     };
@@ -550,14 +560,14 @@ k_rfft_x_products(XProdArgs a, int64_t total)
                 double2 u[Q];
                 if (in_a) {
                     const int deriv = itp->deriv;
-                    if (deriv == 0) rbwd_load_a<Q, NB, false>(stg, p, r, M, 0, a.kscale, u);
-                    else rbwd_load_a<Q, NB, true>(stg, p, r, M, deriv, a.kscale, u);
-                    rbwd_exchange_a<Q, NB>(u, X, a.twn, p, r);
+                    if (deriv == 0) rbwd_load_a<Q, NB, P, false>(stg, p, r, M, 0, a.kscale, u);
+                    else rbwd_load_a<Q, NB, P, true>(stg, p, r, M, deriv, a.kscale, u);
+                    rbwd_exchange_a<Q, NB, P>(u, X, a.twn, p, r);
                 }
                 __syncthreads();                           // staging consumed, exchange written
                 issue();
                 db_cp_commit();
-                if (in_b) rbwd_stage_b<Q, NB>(X, p, r, v);
+                if (in_b) rbwd_stage_b<Q, NB, P>(X, p, r, v);
             }
             const db_xprod_item it = *itp;                 // (read after the transform: not live across it)
             if (in_b) {
@@ -586,7 +596,7 @@ k_rfft_x_products(XProdArgs a, int64_t total)
                     for (int m = 0; m < H; ++m) { X[(k1 + NA * (2 * m + h)) * P + p] = acc[m]; acc[m] = make_double2(0.0, 0.0); }
                 }
                 __syncthreads();
-                rfwd_tile<Q, NB>(X, p, r, fa, [&] { return OutCol{a.out + it.out * a.out_stride + t * (2 * P) + 2 * p, 0}; });
+                rfwd_tile<Q, NB, P>(X, p, r, fa, [&] { return OutCol{a.out + it.out * a.out_stride + t * (2 * P) + 2 * p, 0}; });
                 __syncthreads();
             }
         }
@@ -985,64 +995,148 @@ static int regs_num_sms()
 #endif
 }
 
-template <int Q, int NB>
-int launch_regs(bool fwd, const RegArgs& a, int64_t outer, void* stream)
+// Tile heights (line pairs per tile) at n = 192 and 384 of the standalone transforms (DB_FFT_P = 8 | 4) and of the fused x pass
+// (DB_XPROD_P = 8 | 4); shorter lines always take P = 8.  P = 8 is the faster of the two for both (DESIGN section 4).  Read at
+// every launch, so that one process can time the variants against each other.
+static int tile_pairs(const char* env, int n)
 {
-    constexpr int NA = 3 * Q, THREADS = RegGeom<Q, NB>::THREADS;
-    const size_t bytes = (size_t)2 * NA * NB * RR_P * sizeof(double2);
-    TileWalk w;
-    w.tiles_per_outer = a.inner / (2 * RR_P);
-    w.total = w.tiles_per_outer * outer;
-    // persistent grid: as many CTAs as fit (2 per SM at n = 384: 96 KB each), never more than there are tiles
-    int per_sm = (int)((size_t)(226 * 1024) / (bytes + 1024));
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > 8) per_sm = 8;
-    int64_t nblk = (int64_t)regs_num_sms() * per_sm;
-    if (nblk > w.total) nblk = w.total;
-    dim3 grid((unsigned)nblk);
+    const char* e = n >= 192 && n <= 384 ? getenv(env) : nullptr;
+    return e && atoi(e) == 4 ? 4 : 8;
+}
+
+// CTAs of `kern` resident on one SM: the persistent grids launch exactly this many per SM (more would run as a second wave)
+template <class K> int resident_per_sm(K kern, int threads, size_t bytes, int fit)
+{
+#ifdef DB_EMU
+    (void)kern; (void)threads; (void)bytes;
+    return fit;
+#else
+    int nb = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, threads, bytes) != cudaSuccess || nb < 1) return fit;
+    return nb;
+#endif
+}
+
+template <int Q, int NB, int P>
+size_t regs_smem() { return (size_t)2 * 3 * Q * NB * P * sizeof(double2); }
+
+template <int Q, int NB, int P>
+void regs_attrs()
+{
 #ifndef DB_EMU
     static bool attr = false;
     if (!attr) {
-        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
-        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
-        cudaFuncSetAttribute(k_rfwd_regs<Q, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
-        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-        cudaFuncSetAttribute(k_rfwd_regs<Q, NB>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, P, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
+        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, P, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
+        cudaFuncSetAttribute(k_rfwd_regs<Q, NB, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
+        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, P, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        cudaFuncSetAttribute(k_rbwd_regs<Q, NB, P, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        cudaFuncSetAttribute(k_rfwd_regs<Q, NB, P>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
         attr = true;
     }
 #endif
-    if (fwd) DB_LAUNCH((k_rfwd_regs<Q, NB>), grid, dim3(THREADS), bytes, stream, a, w);
-    else if (a.deriv > 0) DB_LAUNCH((k_rbwd_regs<Q, NB, true>), grid, dim3(THREADS), bytes, stream, a, w);
-    else DB_LAUNCH((k_rbwd_regs<Q, NB, false>), grid, dim3(THREADS), bytes, stream, a, w);
+}
+
+template <int Q, int NB, int P>
+int launch_regs_p(bool fwd, const RegArgs& a, int64_t outer, void* stream)
+{
+    constexpr int THREADS = RegGeom<Q, NB, P>::THREADS;
+    const size_t bytes = regs_smem<Q, NB, P>();
+    TileWalk w;
+    w.tiles_per_outer = a.inner / (2 * P);
+    w.total = w.tiles_per_outer * outer;
+    // persistent grid: as many CTAs as are resident (at n = 384, P = 8: 2 per SM of 96 KB each for the plain backward, 1 for
+    // the forward and derivative backward, which take the whole register file), never more than there are tiles
+    int per_sm = (int)((size_t)(226 * 1024) / (bytes + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 8) per_sm = 8;
+    regs_attrs<Q, NB, P>();
+    if (fwd) per_sm = resident_per_sm(k_rfwd_regs<Q, NB, P>, THREADS, bytes, per_sm);
+    else if (a.deriv > 0) per_sm = resident_per_sm(k_rbwd_regs<Q, NB, P, true>, THREADS, bytes, per_sm);
+    else per_sm = resident_per_sm(k_rbwd_regs<Q, NB, P, false>, THREADS, bytes, per_sm);
+    int64_t nblk = (int64_t)regs_num_sms() * per_sm;
+    if (nblk > w.total) nblk = w.total;
+    dim3 grid((unsigned)nblk);
+    if (fwd) DB_LAUNCH((k_rfwd_regs<Q, NB, P>), grid, dim3(THREADS), bytes, stream, a, w);
+    else if (a.deriv > 0) DB_LAUNCH((k_rbwd_regs<Q, NB, P, true>), grid, dim3(THREADS), bytes, stream, a, w);
+    else DB_LAUNCH((k_rbwd_regs<Q, NB, P, false>), grid, dim3(THREADS), bytes, stream, a, w);
     return db_check_launch(fwd ? "rfft_forward(regs)" : "rfft_backward(regs)");
 }
 
 template <int Q, int NB>
-int launch_x_products(const XProdArgs& a, int32_t n_held, void* stream)
+int launch_regs(bool fwd, const RegArgs& a, int64_t outer, void* stream)
 {
-    using X = XpGeom<Q, NB>;
+    if constexpr (3 * Q * NB >= 192 && 3 * Q * NB <= 384) {
+        if (tile_pairs("DB_FFT_P", 3 * Q * NB) == 4) return launch_regs_p<Q, NB, 4>(fwd, a, outer, stream);
+    }
+    return launch_regs_p<Q, NB, 8>(fwd, a, outer, stream);
+}
+
+// CTAs per SM of the fused x pass (its persistent grid is this times the SM count)
+template <int Q, int NB, int P>
+int x_products_per_sm(size_t bytes)
+{
+    using X = XpGeom<Q, NB, P>;
+    int fit = (int)((size_t)(226 * 1024) / (bytes + 1024));
+    if (fit > X::MINB) fit = X::MINB;
+    if (fit < 1) fit = 1;
+#ifndef DB_EMU
+    static bool attr = false;
+    if (!attr) {
+        cudaFuncSetAttribute(k_rfft_x_products<Q, NB, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
+        cudaFuncSetAttribute(k_rfft_x_products<Q, NB, P>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        attr = true;
+    }
+#endif
+    return resident_per_sm(k_rfft_x_products<Q, NB, P>, X::THREADS, bytes, fit);
+}
+
+template <int Q, int NB, int P>
+int launch_x_products_p(const XProdArgs& a, int32_t n_held, void* stream)
+{
+    using X = XpGeom<Q, NB, P>;
     const size_t bytes = X::smem(a.M, n_held);
     if (bytes > (size_t)DB_MAX_SMEM) {
         db_set_error("rfft_x_products: %d held factors at n = %d need %zu bytes of shared memory", (int)n_held, X::N, bytes);
         return 1;
     }
-    const int64_t total = a.inner / (2 * RR_P);
-    int per_sm = (int)((size_t)(226 * 1024) / (bytes + 1024));
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > 8) per_sm = 8;
-    int64_t nblk = (int64_t)regs_num_sms() * per_sm;
+    const int64_t total = a.inner / (2 * P);
+    int64_t nblk = (int64_t)regs_num_sms() * x_products_per_sm<Q, NB, P>(bytes);
     if (nblk > total) nblk = total;
-#ifndef DB_EMU
-    static bool attr = false;
-    if (!attr) {
-        cudaFuncSetAttribute(k_rfft_x_products<Q, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
-        cudaFuncSetAttribute(k_rfft_x_products<Q, NB>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-        attr = true;
-    }
-#endif
-    DB_LAUNCH((k_rfft_x_products<Q, NB>), dim3((unsigned)nblk), dim3(X::THREADS), bytes, stream, a, total);
+    DB_LAUNCH((k_rfft_x_products<Q, NB, P>), dim3((unsigned)nblk), dim3(X::THREADS), bytes, stream, a, total);
     return db_check_launch("rfft_x_products");
+}
+
+template <int Q, int NB>
+int launch_x_products(const XProdArgs& a, int32_t n_held, void* stream)
+{
+    if constexpr (3 * Q * NB >= 192 && 3 * Q * NB <= 384) {
+        if (tile_pairs("DB_XPROD_P", 3 * Q * NB) == 4) return launch_x_products_p<Q, NB, 4>(a, n_held, stream);
+    }
+    return launch_x_products_p<Q, NB, 8>(a, n_held, stream);
+}
+
+template <int Q, int NB, int P>
+int blocks_per_sm_p(int kind, int32_t n_coeff, int32_t n_held)
+{
+    if (kind == 2) return x_products_per_sm<Q, NB, P>(XpGeom<Q, NB, P>::smem(n_coeff, n_held));
+    regs_attrs<Q, NB, P>();
+    const size_t bytes = regs_smem<Q, NB, P>();
+    int fit = (int)((size_t)(226 * 1024) / (bytes + 1024));
+    fit = fit < 1 ? 1 : (fit > 8 ? 8 : fit);
+    if (kind == 1) return resident_per_sm(k_rfwd_regs<Q, NB, P>, RegGeom<Q, NB, P>::THREADS, bytes, fit);
+    return resident_per_sm(k_rbwd_regs<Q, NB, P, false>, RegGeom<Q, NB, P>::THREADS, bytes, fit);
+}
+
+template <int Q, int NB>
+int blocks_per_sm(int kind, int32_t n_coeff, int32_t n_held, int P)
+{
+    if (kind < 0 || kind > 2) return -1;
+    if (P == 8) return blocks_per_sm_p<Q, NB, 8>(kind, n_coeff, n_held);
+    if constexpr (3 * Q * NB >= 192 && 3 * Q * NB <= 384) {
+        if (P == 4) return blocks_per_sm_p<Q, NB, 4>(kind, n_coeff, n_held);
+    }
+    return -1;
 }
 
 static long long g_regs_launches = 0;
@@ -1062,7 +1156,7 @@ int db_rfft_regs_try(bool fwd, const db_fft_plan* plan, const double* in, double
     if (!enabled) return -1;
     const int n = plan->n;
     if (!plan->half || plan->twn == nullptr) return -1;
-    if (inner < 2 * RR_P || inner % (2 * RR_P) != 0 || deriv > 4) return -1;
+    if (inner < RR_LINES || inner % RR_LINES != 0 || deriv > 4) return -1;
     if (n_coeff % 2 != 0 || n_coeff < 2 || (int64_t)3 * n_coeff > (int64_t)2 * n) return -1;
     if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) return -1;
     RegArgs a;
@@ -1127,7 +1221,7 @@ extern "C" int db_rfft_x_products(const db_fft_plan* plan, const double* in, int
                                   const int32_t* loads, int32_t n_loads, int32_t n_held, void* stream)
 {
     const int n = plan->n;
-    const bool ok = plan->half && plan->twn != nullptr && inner >= 2 * RR_P && inner % (2 * RR_P) == 0 && n_coeff % 2 == 0 &&
+    const bool ok = plan->half && plan->twn != nullptr && inner >= RR_LINES && inner % RR_LINES == 0 && n_coeff % 2 == 0 &&
                     n_coeff >= 2 && (int64_t)3 * n_coeff <= (int64_t)2 * n && n_held >= 0 && n_held <= 3 && n_items > 0 &&
                     n_loads > 0 && in_stride % 2 == 0 && out_stride % 2 == 0 &&
                     ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
@@ -1150,5 +1244,19 @@ extern "C" int db_rfft_x_products(const db_fft_plan* plan, const double* in, int
             --g_regs_launches;
             db_set_error("rfft_x_products: no kernel for n = %d", n);
             return 1;
+    }
+}
+
+// Resident CTAs per SM of a register transform (kind 0: backward, 1: forward) or of the fused x pass (kind 2, with n_coeff rows
+// and n_held held factors) at n grid points and `tile_pairs` line pairs per tile; -1 where no such kernel exists.
+extern "C" int db_rfft_blocks_per_sm(int32_t kind, int32_t n, int32_t n_coeff, int32_t n_held, int32_t tile_pairs)
+{
+    switch (n) {
+        case 384: return blocks_per_sm<8, 16>(kind, n_coeff, n_held, tile_pairs);
+        case 192: return blocks_per_sm<4, 16>(kind, n_coeff, n_held, tile_pairs);
+        case 96:  return blocks_per_sm<4, 8>(kind, n_coeff, n_held, tile_pairs);
+        case 48:  return blocks_per_sm<2, 8>(kind, n_coeff, n_held, tile_pairs);
+        case 24:  return blocks_per_sm<2, 4>(kind, n_coeff, n_held, tile_pairs);
+        default: return -1;
     }
 }

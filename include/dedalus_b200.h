@@ -167,6 +167,10 @@ typedef struct { double coef; int32_t src; int32_t deriv; int32_t a; int32_t b; 
 int db_rfft_x_products(const db_fft_plan* plan, const double* in, int64_t in_stride, double* out, int64_t out_stride,
                        int32_t n_coeff, int64_t inner, double kscale, const db_xprod_item* items, int32_t n_items,
                        const int32_t* loads, int32_t n_loads, int32_t n_held, void* stream);
+/* CTAs resident per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor on the current device) of the register real-Fourier
+ * transforms at n grid points with tile_pairs line pairs per tile: kind 0 backward, 1 forward, 2 the fused x pass with n_coeff
+ * rows and n_held held factors (its persistent grid is this many CTAs per SM).  -1 where there is no such kernel. */
+int db_rfft_blocks_per_sm(int32_t kind, int32_t n, int32_t n_coeff, int32_t n_held, int32_t tile_pairs);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Pencil systems (S1-S4).  A batch holds S structurally identical systems of size n; one thread owns one system.

@@ -6,7 +6,7 @@ so = pathlib.Path(__file__).resolve().parents[1] / "dedalus_b200" / "libdedalus_
 out = subprocess.run(["cuobjdump", "-sass", str(so)], capture_output=True, text=True).stdout
 WANT = ["UBLKCP", "SYNCS", "LDGSTS", "DMMA", "DFMA", "DADD", "DMUL", "LDS", "STS", "LDG", "LD.E", "STG", "ST.E", "BAR", "SHFL", "CCTL", "FSEL", "BRA"]
 KERNELS = ["k_batches_solve_ws", "k_batches_solve_flat", "k_batches_solve_deep", "k_batches_matvec", "k_batches_move", "k_batches_factor",
-           "k_batches_residual", "k_rbwd_regs", "k_rfwd_regs", "k_chbwd_regs", "k_chfwd_regs", "k_pointwise_pairs", "k_mmt_dmma",
+           "k_batches_residual", "k_rbwd_regs", "k_rfwd_regs", "k_rfft_x_products", "k_chbwd_regs", "k_chfwd_regs", "k_pointwise_pairs", "k_mmt_dmma",
            "k_ragged_matvec", "k_band_scan2", "k_tr_chunks", "k_cfl_max"]
 cur, counts, total = None, collections.OrderedDict(), {}
 for line in out.splitlines():
@@ -28,7 +28,7 @@ for fn, c in counts.items():
     if not any(k in fn for k in KERNELS):
         continue
     dem = sp.run(["c++filt", fn], capture_output=True, text=True).stdout.strip()
-    dem = re.sub(r"\(.*$", "", dem).replace("void ", "").replace("(anonymous namespace)::", "")
+    dem = re.sub(r"\(.*$", "", dem.replace("(anonymous namespace)::", "")).replace("void ", "")
     if total[fn] < 40:
         continue
     print(f"| `{dem[:60]}` | {total[fn]} | " + " | ".join(str(c.get(w, 0)) for w in WANT) + " |")
