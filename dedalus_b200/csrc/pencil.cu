@@ -314,29 +314,16 @@ __device__ __forceinline__ int find_batch(const db_batch* __restrict__ b, int nb
 // ---------------------------------------------------------------------------------------------------------
 #define SOLVE_CE 16
 #ifdef DB_EMU
-// test emulation: low 32 bits = bytes still expected, high 32 bits = completed phases; copies complete at issue, and a
-// waiter yields to the other fibers until the phase it waits for is complete (threads may run ahead of the producer)
+// test emulation (tests/emu/cuda_emu.h): bulk copies are queued on their mbarrier and land when a thread waits on it
+// (DB_EMU_BULK=late) or at issue (early); a waiter yields to the other fibers until the phase it waits for is complete
 typedef unsigned long long db_mbar_t;
-__device__ __forceinline__ void db_mbar_init(db_mbar_t* bar, int) { *bar = 0; }
+__device__ __forceinline__ void db_mbar_init(db_mbar_t* bar, int) { emu_mbar_init(bar); }
 __device__ __forceinline__ void db_mbar_fence_init() {}
-__device__ __forceinline__ void db_mbar_expect_tx(db_mbar_t* bar, unsigned bytes) { *bar += bytes; }
-__device__ __forceinline__ void db_bulk_g2s(void* dst, const void* src, unsigned bytes, db_mbar_t* bar)
-{
-    memcpy(dst, src, bytes);
-    *bar -= bytes;
-    if ((*bar & 0xffffffffull) == 0) *bar += 1ull << 32;
-}
-__device__ __forceinline__ void db_mbar_wait(db_mbar_t* bar, unsigned parity)
-{
-    while ((((*bar) >> 32) & 1ull) == parity) emu_yield();
-}
-// arrival-count barrier (emulation): bits 0-15 pending arrivals, bits 16-31 arrivals per phase, bits 32.. completed phases
-__device__ __forceinline__ void db_cbar_init(db_mbar_t* bar, int count) { *bar = (unsigned long long)count | ((unsigned long long)count << 16); }
-__device__ __forceinline__ void db_cbar_arrive(db_mbar_t* bar)
-{
-    *bar -= 1;
-    if ((*bar & 0xffffull) == 0) *bar += (1ull << 32) + ((*bar >> 16) & 0xffffull);
-}
+__device__ __forceinline__ void db_mbar_expect_tx(db_mbar_t* bar, unsigned bytes) { emu_mbar_expect_tx(bar, bytes); }
+__device__ __forceinline__ void db_bulk_g2s(void* dst, const void* src, unsigned bytes, db_mbar_t* bar) { emu_bulk_g2s(dst, src, bytes, bar); }
+__device__ __forceinline__ void db_mbar_wait(db_mbar_t* bar, unsigned parity) { emu_mbar_wait(bar, parity); }
+__device__ __forceinline__ void db_cbar_init(db_mbar_t* bar, int count) { emu_cbar_init(bar, count); }
+__device__ __forceinline__ void db_cbar_arrive(db_mbar_t* bar) { emu_cbar_arrive(bar); }
 #define DB_CBAR_PER_THREAD 1        // every consumer thread arrives (fibers are not warp-synchronous)
 #else
 typedef unsigned long long db_mbar_t;
@@ -965,11 +952,39 @@ k_batches_solve_deep(const db_batch* __restrict__ batches, int nbatch, int lu_sl
     }
 }
 
+// Run-time choice of the solve kernel and its ring (db_batches_solve_set_mode); a negative field keeps the environment's choice.
+// Kernels: 0 k_batches_solve_ws, 1 _flat, 2 _pipe, 3 _mr<2>, 4 _mr<4>, 5 _deep.
+static int g_sv_kernel = -1, g_sv_stages = -1, g_sv_cps = -1, g_sv_minb = -1, g_sv_pf = -1, g_sv_mpc = -1;
+#define SOLVE_WS_SMEM(nst, cps) ((size_t)(nst) * (cps) * SOLVE_FSTAGE_BYTES + (size_t)2 * (nst) * sizeof(db_mbar_t))
+
+extern "C" int db_batches_solve_set_mode(int32_t kernel, int32_t stages, int32_t chunks_per_stage, int32_t minb, int32_t prefetch,
+                                         int32_t deep_members)
+{
+    if (kernel > 5 || (stages >= 0 && (stages < 2 || stages > 24)) || chunks_per_stage == 0 || chunks_per_stage > 8 || minb == 0 ||
+        minb > 4 || prefetch > 2 || (deep_members >= 0 && deep_members != 1 && deep_members != 2 && deep_members != 4)) {
+        db_set_error("batches_solve_set_mode: argument out of range (kernel %d, stages %d, chunks per stage %d, minb %d, prefetch %d, "
+                     "deep members %d)", kernel, stages, chunks_per_stage, minb, prefetch, deep_members);
+        return 1;
+    }
+    if (kernel == 5 && stages >= 0 && stages < SOLVE_DEEP_D + 2) {
+        db_set_error("batches_solve_set_mode: the deep kernel needs at least %d stages", SOLVE_DEEP_D + 2); return 1;
+    }
+    if (kernel == 0 && stages >= 0 && chunks_per_stage > 0 && SOLVE_WS_SMEM(stages, chunks_per_stage) > DB_MAX_SMEM) {
+        db_set_error("batches_solve_set_mode: %d stages of %d chunks need %zu bytes of shared memory (limit %d)", stages,
+                     chunks_per_stage, SOLVE_WS_SMEM(stages, chunks_per_stage), DB_MAX_SMEM);
+        return 1;
+    }
+    g_sv_kernel = kernel; g_sv_stages = stages; g_sv_cps = chunks_per_stage; g_sv_minb = minb; g_sv_pf = prefetch; g_sv_mpc = deep_members;
+    return 0;
+}
+
 extern "C" int db_batches_solve(const db_batch* batches, int32_t nbatch, int32_t total_blocks, int32_t max_nrhs, int32_t lu_slot, int32_t x_slot,
                                 const db_slotcomb* rhs, void* stream)
 {
     if (nbatch <= 0 || total_blocks <= 0) return 0;
-    if (rhs->nvec < 0 || rhs->nvec > 16 || lu_slot < 0 || lu_slot >= DB_MAX_LU || max_nrhs < 1 || max_nrhs > SOLVE_MAX_RHS) {
+    // nvec >= 1: the kernels pad the combination to their template size with zero-coefficient copies of the first term, so an
+    // empty one would give 0 * vec[slot[0]] (NaN where that slot holds NaN) in some variants and 0 in others
+    if (rhs->nvec < 1 || rhs->nvec > 16 || lu_slot < 0 || lu_slot >= DB_MAX_LU || max_nrhs < 1 || max_nrhs > SOLVE_MAX_RHS) {
         db_set_error("batches_solve: bad arguments"); return 1;
     }
     const dim3 g(total_blocks), b(SOLVE_THREADS * max_nrhs);
@@ -986,55 +1001,72 @@ extern "C" int db_batches_solve(const db_batch* batches, int32_t nbatch, int32_t
         const char* c = getenv("DB_SOLVE_CPS"); cps_env = c ? atoi(c) : 2;
         if (cps_env < 1 || cps_env > 8) cps_env = 2;
     }
+    // fields set by db_batches_solve_set_mode replace the environment's
+    const int st_sel = g_sv_stages >= 0 ? g_sv_stages : st_env;
+    const int cps = g_sv_cps > 0 ? g_sv_cps : cps_env, minb = g_sv_minb > 0 ? g_sv_minb : minb_env, pf = g_sv_pf >= 0 ? g_sv_pf : pf_env;
     // ring depth: with ~7 CTAs per SM two stages already keep 100+ KB of factor bytes in flight per SM and every
     // further stage only shrinks the L1 the x gathers live in; with few CTAs per SM the ring is the only source of
     // memory parallelism, so it gets deep
     const int per_sm = (total_blocks + db_num_sms() - 1) / db_num_sms();
     int nst = per_sm >= 5 ? 2 : per_sm >= 3 ? 4 : per_sm >= 2 ? 8 : 16;
-    if (st_env >= 2 && st_env <= 24) nst = st_env;
+    if (st_sel >= 2 && st_sel <= 24) nst = st_sel;
     const size_t smem = (size_t)nst * SOLVE_FSTAGE_BYTES + (size_t)nst * sizeof(db_mbar_t);
     // members per thread: 1 = k_batches_solve_flat; 2 / 4 = k_batches_solve_mr (RT chains per thread; opt-in, DB_SOLVE_RT)
     int rt = rt_env ? rt_env : 1;       // 2 and 4 leave fewer resident warps
     if (rt != 1 && rt != 2 && rt != 4) rt = 1;
     if (rt > max_nrhs) rt = max_nrhs >= 2 ? 2 : 1;
-    const dim3 bmr(SOLVE_THREADS * ((max_nrhs + rt - 1) / rt));
     // deep-prefetch kernel: by default when there is at most one tile per SM (the launch is then bound by one thread's
     // dependent chain, not by bandwidth); DB_SOLVE_DEEP = 0 / 1 forces it off / on.  Members per CTA: as few as still give
     // at most one CTA per SM (more SMs at work, deeper factor ring per CTA); DB_SOLVE_DEEP_MPC overrides.
     const bool deep = deep_env > 0;          // opt-in (DB_SOLVE_DEEP=1)
+    int kern = g_sv_kernel;
+    if (kern < 0) kern = (ws_env && !deep && rt == 1 && !pipe_env) ? 0 : deep ? 5 : (rt == 4 && !pipe_env) ? 4 : (rt == 2 && !pipe_env) ? 3
+                       : pipe_env ? 2 : 1;
+    else if (kern == 3 || kern == 4) rt = kern == 3 ? 2 : 4;      // as asked: the work vectors hold whole groups of 4 members
+    const dim3 bmr(SOLVE_THREADS * ((max_nrhs + rt - 1) / rt));
     static int mpc_env = -1;
     if (mpc_env < 0) { const char* e = getenv("DB_SOLVE_DEEP_MPC"); mpc_env = e ? atoi(e) : 0; }
+    const int mpc_sel = g_sv_mpc > 0 ? g_sv_mpc : mpc_env;
     int mpc = 1;
     while (mpc < max_nrhs && total_blocks * ((max_nrhs + mpc - 1) / mpc) > db_num_sms()) mpc *= 2;
-    if (mpc_env == 1 || mpc_env == 2 || mpc_env == 4) mpc = mpc_env;
+    if (mpc_sel == 1 || mpc_sel == 2 || mpc_sel == 4) mpc = mpc_sel;
     if (mpc > max_nrhs) mpc = max_nrhs;
     const dim3 g_deep(total_blocks, (max_nrhs + mpc - 1) / mpc), b_deep(SOLVE_THREADS * mpc);
     const size_t deep_fixed = (size_t)((SOLVE_DEEP_D + 1) * SOLVE_CE + SOLVE_DEEP_RRN) * b_deep.x * sizeof(double) + 64;
     int nst_deep = (int)(((size_t)220 * 1024 - deep_fixed) / (SOLVE_FSTAGE_BYTES + sizeof(db_mbar_t)));
     if (nst_deep > 24) nst_deep = 24;
-    if (st_env >= SOLVE_DEEP_D + 2 && st_env <= 24 && st_env < nst_deep) nst_deep = st_env;
+    if (kern == 5 && g_sv_stages >= 0 && g_sv_stages > nst_deep) {
+        db_set_error("batches_solve: %d stages of the deep kernel do not fit in shared memory next to %d members per CTA (at most %d)",
+                     g_sv_stages, mpc, nst_deep);
+        return 1;
+    }
+    if (st_sel >= SOLVE_DEEP_D + 2 && st_sel <= 24 && (st_sel < nst_deep || st_sel == g_sv_stages)) nst_deep = st_sel;
     const size_t smem_deep = (((size_t)nst_deep * SOLVE_FSTAGE_BYTES + (size_t)nst_deep * sizeof(db_mbar_t) + 15) & ~(size_t)15) + deep_fixed;
+    int nst_ws = (nst * 1 + cps - 1) / cps; if (nst_ws < 3) nst_ws = 3;
+    if (st_sel >= 2 && st_sel <= 24) nst_ws = st_sel;
+    const size_t smem_ws = SOLVE_WS_SMEM(nst_ws, cps);
+    if (kern == 0 && smem_ws > DB_MAX_SMEM) {
+        db_set_error("batches_solve: %d stages of %d chunks need %zu bytes of shared memory (limit %d)", nst_ws, cps, smem_ws, DB_MAX_SMEM);
+        return 1;
+    }
 #define FLAT_GO(NV_) { static int attr_st = 0; \
     if (!attr_st) { DB_SET_SMEM_ATTR((k_batches_solve_flat<NV_, 2>)); DB_SET_SMEM_ATTR((k_batches_solve_flat<NV_, 3>)); DB_SET_SMEM_ATTR((k_batches_solve_flat<NV_, 4>)); \
                     DB_SET_SMEM_ATTR((k_batches_solve_pipe<NV_>)); \
                     DB_SET_SMEM_ATTR((k_batches_solve_mr<NV_, 2>)); DB_SET_SMEM_ATTR((k_batches_solve_mr<NV_, 4>)); \
                     DB_SET_SMEM_ATTR((k_batches_solve_ws<NV_, 1>)); DB_SET_SMEM_ATTR((k_batches_solve_ws<NV_, 2>)); DB_SET_SMEM_ATTR((k_batches_solve_ws<NV_, 3>)); \
                     DB_SET_SMEM_ATTR((k_batches_solve_deep<NV_>)); attr_st = 1; } \
-    if (ws_env && !deep && rt == 1 && !pipe_env) { \
-        int nst_ws = (nst * 1 + cps_env - 1) / cps_env; if (nst_ws < 3) nst_ws = 3; \
-        if (st_env >= 2 && st_env <= 24) nst_ws = st_env; \
-        const size_t smem_ws = (size_t)nst_ws * cps_env * SOLVE_FSTAGE_BYTES + (size_t)2 * nst_ws * sizeof(db_mbar_t); \
-        const int code = nst_ws | (pf_env << 8) | (cps_env << 16); \
-        if (minb_env == 4) DB_LAUNCH((k_batches_solve_ws<NV_, 3>), g, dim3(b.x + 32), smem_ws, stream, batches, nbatch, lu_slot, x_slot, *rhs, code); \
-        else if (minb_env == 1) DB_LAUNCH((k_batches_solve_ws<NV_, 1>), g, dim3(b.x + 32), smem_ws, stream, batches, nbatch, lu_slot, x_slot, *rhs, code); \
+    if (kern == 0) { \
+        const int code = nst_ws | (pf << 8) | (cps << 16); \
+        if (minb == 4) DB_LAUNCH((k_batches_solve_ws<NV_, 3>), g, dim3(b.x + 32), smem_ws, stream, batches, nbatch, lu_slot, x_slot, *rhs, code); \
+        else if (minb == 1) DB_LAUNCH((k_batches_solve_ws<NV_, 1>), g, dim3(b.x + 32), smem_ws, stream, batches, nbatch, lu_slot, x_slot, *rhs, code); \
         else DB_LAUNCH((k_batches_solve_ws<NV_, 2>), g, dim3(b.x + 32), smem_ws, stream, batches, nbatch, lu_slot, x_slot, *rhs, code); } \
-    else if (deep) DB_LAUNCH((k_batches_solve_deep<NV_>), g_deep, b_deep, smem_deep, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst_deep | (pf_env << 8)); \
-    else if (rt == 4 && !pipe_env) DB_LAUNCH((k_batches_solve_mr<NV_, 4>), g, bmr, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst); \
-    else if (rt == 2 && !pipe_env) DB_LAUNCH((k_batches_solve_mr<NV_, 2>), g, bmr, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst); \
-    else if (pipe_env && nst >= 2) DB_LAUNCH((k_batches_solve_pipe<NV_>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst); \
-    else if (minb_env == 4) DB_LAUNCH((k_batches_solve_flat<NV_, 4>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst | (pf_env << 8)); \
-    else if (minb_env == 2) DB_LAUNCH((k_batches_solve_flat<NV_, 2>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst | (pf_env << 8)); \
-    else DB_LAUNCH((k_batches_solve_flat<NV_, 3>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst | (pf_env << 8)); }
+    else if (kern == 5) DB_LAUNCH((k_batches_solve_deep<NV_>), g_deep, b_deep, smem_deep, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst_deep | (pf << 8)); \
+    else if (kern == 4) DB_LAUNCH((k_batches_solve_mr<NV_, 4>), g, bmr, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst); \
+    else if (kern == 3) DB_LAUNCH((k_batches_solve_mr<NV_, 2>), g, bmr, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst); \
+    else if (kern == 2) DB_LAUNCH((k_batches_solve_pipe<NV_>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst); \
+    else if (minb == 4) DB_LAUNCH((k_batches_solve_flat<NV_, 4>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst | (pf << 8)); \
+    else if (minb == 2) DB_LAUNCH((k_batches_solve_flat<NV_, 2>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst | (pf << 8)); \
+    else DB_LAUNCH((k_batches_solve_flat<NV_, 3>), g, b, smem, stream, batches, nbatch, lu_slot, x_slot, *rhs, nst | (pf << 8)); }
     if (nv <= 1) FLAT_GO(1) else if (nv == 2) FLAT_GO(2) else if (nv == 3) FLAT_GO(3) else if (nv == 4) FLAT_GO(4)
     else if (nv == 5) FLAT_GO(5) else if (nv == 6) FLAT_GO(6) else if (nv <= 8) FLAT_GO(8) else if (nv <= 12) FLAT_GO(12) else FLAT_GO(16)
 #undef FLAT_GO

@@ -105,6 +105,7 @@ SIGNATURES = {
     "db_batches_move": (C.c_int, [vp, i32, i32, i32, i32, i32, vp, vp]),
     "db_batches_matvec": (C.c_int, [vp, i32, i32, i32, i32, i32, vp]),
     "db_batches_solve": (C.c_int, [vp, i32, i32, i32, i32, i32, C.c_void_p, vp]),
+    "db_batches_solve_set_mode": (C.c_int, [i32, i32, i32, i32, i32, i32]),
     "db_batches_assemble": (C.c_int, [vp, i32, i32, i32, vp]),
     "db_batches_factor": (C.c_int, [vp, i32, i32, i32, vp]),
     "db_batches_residual": (C.c_int, [vp, i32, i32, i32, i32, i32, f64, f64, vp, vp]),

@@ -289,10 +289,18 @@ int db_batches_move(const db_batch* batches, int32_t nbatch, int32_t total_block
                     int32_t slot, double* arena, void* stream);
 /* vec[ym_slot] = M vec[x_slot], vec[yl_slot] = L vec[x_slot]; a negative slot skips that product */
 int db_batches_matvec(const db_batch* batches, int32_t nbatch, int32_t total_blocks, int32_t x_slot, int32_t ym_slot, int32_t yl_slot, void* stream);
-/* vec[x_slot] = LU[lu_slot]^{-1} (sum_j coef[j] vec[slot[j]]) */
+/* vec[x_slot] = LU[lu_slot]^{-1} (sum_j coef[j] vec[slot[j]]), 1 <= nvec <= 16 */
 /* max_nrhs: largest db_batch.nrhs of the set (the CTAs have 64 * max_nrhs threads) */
 int db_batches_solve(const db_batch* batches, int32_t nbatch, int32_t total_blocks, int32_t max_nrhs, int32_t lu_slot, int32_t x_slot,
                      const db_slotcomb* rhs, void* stream);
+/* Kernel and ring of db_batches_solve for this process (also environment DB_SOLVE_WS / _PIPE / _RT / _DEEP / _STAGES / _CPS /
+ * _MINB / _PF / _DEEP_MPC, read once).  kernel: 0 warp-specialised ring (default), 1 flat, 2 pipelined gathers, 3 / 4 two / four
+ * members per thread (these solve whole groups of 2 / 4 members: the work vectors must hold them), 5 deep prefetch.  stages: ring
+ * depth, 2 .. 24 (deep: at least 5); chunks_per_stage: 1 .. 8 (warp-specialised ring only); minb: 1 .. 4, the CTAs per SM the
+ * register budget is built for; prefetch: 0 none, 1 L2, 2 L1 prefetch of row start values; deep_members: 1, 2 or 4 members per
+ * CTA of the deep kernel.  All variants give bitwise-equal results.  A negative field returns to the environment's choice.
+ * Out-of-range values, and rings that do not fit in shared memory, are rejected (here or by the next solve) with an error. */
+int db_batches_solve_set_mode(int32_t kernel, int32_t stages, int32_t chunks_per_stage, int32_t minb, int32_t prefetch, int32_t deep_members);
 /* LU[lu_slot] = assembled LHS (asm_* programs), then in-place factorisation */
 int db_batches_assemble(const db_batch* batches, int32_t nbatch, int32_t total_blocks, int32_t lu_slot, void* stream);
 int db_batches_factor(const db_batch* batches, int32_t nbatch, int32_t total_blocks, int32_t lu_slot, void* stream);

@@ -1,5 +1,7 @@
 // TEST INFRASTRUCTURE ONLY: fiber scheduler for tests/emu/cuda_emu.h
 #include "cuda_emu.h"
+#include <cstdarg>
+#include <cstdint>
 #include <stdexcept>
 
 thread_local EmuState emu_cur;
@@ -15,6 +17,8 @@ struct Fiber {
     EmuState st;
     bool done = false;
     bool created = false;
+    const char* wait_what = nullptr;                    // set when the fiber last yielded from an emulated wait (deadlock detection)
+    const void* wait_on = nullptr;
 };
 const size_t STACK = 128 * 1024;
 thread_local Fiber fiber_pool[1024];                    // a block has at most 1024 threads
@@ -55,6 +59,16 @@ void emu_yield() {
     emu_cur = f->st;
 }
 
+// every change of barrier or copy-queue state counts here: a scheduling round in which it stays put while every live fiber
+// waits is a deadlock
+static thread_local size_t emu_progress = 0;
+// a yield from inside an emulated wait: records what the fiber waits for
+static void emu_wait_yield(const char* what, const void* on) {
+    running->wait_what = what;
+    running->wait_on = on;
+    emu_yield();
+}
+
 // block barrier: a real arrival count (threads that already exited count as arrived, as on the GPU), so that code
 // between two barriers may yield a different number of times in different warps (warp shuffles, see below)
 static thread_local size_t bar_arrived = 0, bar_generation = 0, bar_live = 0;
@@ -64,8 +78,9 @@ static void bar_release_if_complete() {
 void emu_syncthreads() {
     const size_t gen = bar_generation;
     ++bar_arrived;
+    ++emu_progress;
     bar_release_if_complete();
-    while (bar_generation == gen) emu_yield();
+    while (bar_generation == gen) emu_wait_yield("__syncthreads", nullptr);
 }
 
 static double shfl_slots[2][4096];
@@ -126,7 +141,103 @@ void emu_cp_wait(int n) {
     if (q.head == q.copies.size()) { q.copies.clear(); q.head = 0; }
 }
 
-void emu_launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>& body) {
+// mbarriers and bulk copies.  Copies queued under DB_EMU_BULK=late, in issue order; a wait on a barrier lands that barrier's copies.
+namespace {
+struct BulkCopy { unsigned long long* bar; void* dst; const void* src; unsigned bytes; };
+thread_local std::vector<BulkCopy> bulk_queue;
+bool bulk_late() {
+    static const bool late = [] {
+        const char* e = getenv("DB_EMU_BULK");
+        if (!e || !strcmp(e, "late")) return true;
+        if (!strcmp(e, "early")) return false;
+        fprintf(stderr, "DB_EMU_BULK=%s: expected 'late' or 'early'\n", e);
+        abort();
+    }();
+    return late;
+}
+[[noreturn]] void emu_fail(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
+void emu_fail(const char* fmt, ...) {
+    const EmuState& s = emu_cur;
+    fprintf(stderr, "emu: block (%u,%u,%u) thread (%u,%u,%u): ", s.bid.x, s.bid.y, s.bid.z, s.tid.x, s.tid.y, s.tid.z);
+    va_list ap;
+    va_start(ap, fmt);
+    vfprintf(stderr, fmt, ap);
+    va_end(ap);
+    fputc('\n', stderr);
+    abort();
+}
+void check_bar(const unsigned long long* bar, const char* what) {
+    if ((uintptr_t)bar % 8) emu_fail("%s: mbarrier %p is not 8-byte aligned", what, (const void*)bar);
+}
+// one copy lands: its bytes complete on the barrier; the phase completes when none are left
+void bulk_land(const BulkCopy& c) {
+    std::memcpy(c.dst, c.src, c.bytes);
+    const unsigned pending = (unsigned)(*c.bar & 0xffffffffull);
+    if (c.bytes > pending)
+        emu_fail("bulk copy of %u bytes completes on mbarrier %p, which expects only %u more bytes in this phase", c.bytes, (void*)c.bar, pending);
+    *c.bar -= c.bytes;
+    ++emu_progress;
+    if (pending == c.bytes) {
+        for (const BulkCopy& o : bulk_queue)
+            if (o.bar == c.bar) emu_fail("mbarrier %p completed its phase with a %u-byte bulk copy still in flight", (void*)c.bar, o.bytes);
+        *c.bar += 1ull << 32;
+    }
+}
+}  // namespace
+
+void emu_mbar_init(unsigned long long* bar) {
+    check_bar(bar, "mbarrier.init");
+    *bar = 0;
+    ++emu_progress;
+}
+
+void emu_mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
+    check_bar(bar, "mbarrier.arrive.expect_tx");
+    *bar += bytes;
+    ++emu_progress;
+}
+
+void emu_bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {
+    check_bar(bar, "cp.async.bulk");
+    if ((uintptr_t)dst % 16 || (uintptr_t)src % 16) emu_fail("cp.async.bulk: addresses %p <- %p are not 16-byte aligned", dst, src);
+    if (bytes == 0 || bytes % 16) emu_fail("cp.async.bulk: size %u is not a non-zero multiple of 16", bytes);
+    const BulkCopy c{bar, dst, src, bytes};
+    if (bulk_late()) { bulk_queue.push_back(c); ++emu_progress; }
+    else bulk_land(c);
+}
+
+void emu_mbar_wait(unsigned long long* bar, unsigned parity) {
+    check_bar(bar, "mbarrier.try_wait");
+    while (((*bar >> 32) & 1ull) == parity) {
+        // land this barrier's queued copies, oldest first
+        bool landed = false;
+        for (size_t i = 0; i < bulk_queue.size();) {
+            if (bulk_queue[i].bar != bar) { ++i; continue; }
+            const BulkCopy c = bulk_queue[i];
+            bulk_queue.erase(bulk_queue.begin() + i);
+            bulk_land(c);
+            landed = true;
+        }
+        if (!landed) emu_wait_yield("mbarrier", bar);
+    }
+}
+
+// arrival-count barrier: bits 0-15 pending arrivals, bits 16-31 arrivals per phase, bits 32.. completed phases
+void emu_cbar_init(unsigned long long* bar, int count) {
+    check_bar(bar, "mbarrier.init");
+    *bar = (unsigned long long)count | ((unsigned long long)count << 16);
+    ++emu_progress;
+}
+
+void emu_cbar_arrive(unsigned long long* bar) {
+    check_bar(bar, "mbarrier.arrive");
+    if ((*bar & 0xffffull) == 0) emu_fail("mbarrier.arrive on %p: more arrivals than the barrier counts", (void*)bar);
+    *bar -= 1;
+    if ((*bar & 0xffffull) == 0) *bar += (1ull << 32) + ((*bar >> 16) & 0xffffull);
+    ++emu_progress;
+}
+
+void emu_launch(dim3 grid, dim3 block, size_t smem, const char* name, const std::function<void()>& body) {
     const size_t nthreads = (size_t)block.x * block.y * block.z;
     // the launch limits of the real device (sm_90): a launch that violates them fails on the GPU with "invalid configuration
     // argument" while a host loop would just run zero or too many iterations
@@ -150,6 +261,7 @@ void emu_launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>&
         std::memset(shfl_parity, 0, sizeof(shfl_parity));
         // copies still pending when a thread of the previous block exited never land in this block's shared memory
         for (size_t t = 0; t < nthreads; ++t) cp_queues[t].reset();
+        bulk_queue.clear();
         size_t i = 0;
         for (unsigned tz = 0; tz < block.z; ++tz)
         for (unsigned ty = 0; ty < block.y; ++ty)
@@ -165,12 +277,23 @@ void emu_launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>&
         // lower-numbered thread happens to run first (a missing __syncthreads / __syncwarp) passes in one order and fails in the other.
         static const bool reverse_order = [] { const char* e = getenv("DB_EMU_ORDER"); return e && e[0] == 'r'; }();
         while (remaining) {
-            size_t finished_this_round = 0, waiting = 0;
+            size_t finished_this_round = 0, waiting = 0, blocked = 0;
+            const size_t progress0 = emu_progress;
+            const Fiber* first_blocked = nullptr;
             for (size_t fi = 0; fi < nthreads; ++fi) {
                 Fiber& f = fibers[reverse_order ? nthreads - 1 - fi : fi];
                 if (f.done) continue;
+                f.wait_what = nullptr;
                 resume(f);
                 if (f.done) { ++finished_this_round; --bar_live; bar_release_if_complete(); } else { ++waiting; }
+                if (!f.done && f.wait_what) { ++blocked; if (!first_blocked) first_blocked = &f; }
+            }
+            if (!finished_this_round && blocked == waiting && emu_progress == progress0) {
+                const EmuState& s = first_blocked->st;
+                fprintf(stderr, "emu_launch: deadlock in %s: block (%u,%u,%u) has %zu live threads, all waiting, and a whole round changed "
+                        "nothing; thread (%u,%u,%u) waits at %s %p\n", name, s.bid.x, s.bid.y, s.bid.z, waiting, s.tid.x, s.tid.y, s.tid.z,
+                        first_blocked->wait_what, first_blocked->wait_on);
+                abort();
             }
             remaining -= finished_this_round;
             if (finished_this_round && waiting) {

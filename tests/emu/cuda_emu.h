@@ -74,9 +74,24 @@ void emu_cp_async(void* dst, const void* src, size_t bytes);
 void emu_cp_commit();                // close the open group (also when it is empty), as cp.async.commit_group
 void emu_cp_wait(int n);             // land every committed group except the n most recent, as cp.async.wait_group n
 
-void emu_launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>& body);
+// mbarriers and 1-D bulk copies (cp.async.bulk ... mbarrier::complete_tx::bytes).  A barrier is one 64-bit word: low 32 bits = bytes
+// still expected in the current phase (or, for an arrival-count barrier, pending arrivals and arrivals per phase), high 32 bits =
+// completed phases.  With DB_EMU_BULK=late (the default) a bulk copy is queued on its barrier and lands, in issue order, only when a
+// thread waits on that barrier: a stage read before its wait still holds the poison.  With DB_EMU_BULK=early it lands at issue.
+// Either way the PTX rules are enforced (16-byte aligned addresses, a size that is a non-zero multiple of 16, an 8-byte aligned
+// barrier, exactly the expect_tx bytes per phase), and a violation aborts with a message.
+void emu_mbar_init(unsigned long long* bar);
+void emu_mbar_expect_tx(unsigned long long* bar, unsigned bytes);
+void emu_bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar);
+void emu_mbar_wait(unsigned long long* bar, unsigned parity);
+void emu_cbar_init(unsigned long long* bar, int count);
+void emu_cbar_arrive(unsigned long long* bar);
+
+// A launch aborts, naming the block and a waiting thread, when a whole scheduling round passes in which every live thread is
+// blocked in an emulated wait (__syncthreads, mbarrier) and no barrier or copy-queue state changes: on the GPU it would hang.
+void emu_launch(dim3 grid, dim3 block, size_t smem, const char* name, const std::function<void()>& body);
 
 #define DB_LAUNCH(kern, grid, block, smem, stream, ...) \
-    emu_launch(dim3(grid), dim3(block), (size_t)(smem), [&]() { kern(__VA_ARGS__); })
+    emu_launch(dim3(grid), dim3(block), (size_t)(smem), #kern, [&]() { kern(__VA_ARGS__); })
 #define DB_SMEM(type, name) type* name = reinterpret_cast<type*>(emu_cur.smem)
 #define DB_SET_SMEM_ATTR(kern) ((void)0)

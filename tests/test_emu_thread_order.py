@@ -12,7 +12,8 @@ def test_kernels_pass_with_reversed_thread_order():
     env = dict(os.environ, DB_EMU_ORDER="reverse")
     cmd = [sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider",
            str(ROOT / "tests" / "test_emu_shell.py"), str(ROOT / "tests" / "test_emu_sphere.py"), str(ROOT / "tests" / "test_emu_plugins.py"),
-           str(ROOT / "tests" / "test_emu_banded.py"), "-k", "a_sbdf2 or banded or sw16 or matsolver or transforms"]
+           str(ROOT / "tests" / "test_emu_banded.py"), str(ROOT / "tests" / "test_emu_pencil_batches.py"),
+           "-k", "a_sbdf2 or banded or sw16 or matsolver or transforms or pencil_batches"]
     out = subprocess.run(cmd, capture_output=True, text=True, timeout=1200, env=env, cwd=str(ROOT))
     assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-2000:]
     assert " passed" in out.stdout and "failed" not in out.stdout
@@ -37,8 +38,19 @@ def test_cp_async_kernels_pass_with_copies_landing_at_issue():
     tests = ROOT / "tests"
     cmd = [sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider",
            str(tests / "test_emu_banded.py"), str(tests / "test_emu_pencil.py"), str(tests / "test_emu_transforms.py"),
-           str(tests / "test_emu_sphere.py"), str(tests / "test_emu_solver.py"),
-           "-k", "banded or sw16 or pencil_kernels or pointwise or register or benchmark_line or blocked_row or rb3d_steps or pipelined"]
+           str(tests / "test_emu_sphere.py"), str(tests / "test_emu_solver.py"), str(tests / "test_emu_pencil_batches.py"),
+           "-k", "banded or sw16 or pencil_kernels or pointwise or register or benchmark_line or blocked_row or rb3d_steps or pipelined"
+                 " or pencil_batches"]
     out = subprocess.run(cmd, capture_output=True, text=True, timeout=1200, env=dict(os.environ, DB_EMU_CP="early"), cwd=str(ROOT))
+    assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-2000:]
+    assert " passed" in out.stdout and "failed" not in out.stdout
+
+
+def test_pencil_batches_pass_with_bulk_copies_landing_at_issue():
+    """The emulation lands a bulk copy when a thread waits on its mbarrier (DB_EMU_BULK=late, the default), which catches a ring stage
+    read before its wait.  DB_EMU_BULK=early lands it at issue, which catches a stage refilled while it is still being read."""
+    cmd = [sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", str(ROOT / "tests" / "test_emu_pencil_batches.py"),
+           str(ROOT / "tests" / "test_emu_pencil.py"), "-k", "pencil_batches or merged"]
+    out = subprocess.run(cmd, capture_output=True, text=True, timeout=1200, env=dict(os.environ, DB_EMU_BULK="early"), cwd=str(ROOT))
     assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-2000:]
     assert " passed" in out.stdout and "failed" not in out.stdout
