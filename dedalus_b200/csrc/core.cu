@@ -52,31 +52,39 @@ extern "C" int db_device_arch(void)
 #endif
 }
 
-// |x| max reduction: per-block partial maxima combined with atomicMax on the ordered-int representation
+// |x| max reduction: per-block partial maxima combined with atomicMax on the ordered-int representation.  A NaN in the input
+// propagates to the result, as np.max does: it wins every comparison on the way, and is published as the positive quiet NaN,
+// whose bit pattern lies above every finite value and +inf.
+__device__ __forceinline__ void db_publish_max(unsigned long long* out, double v)
+{
+    // non-negative doubles order like their bit patterns
+    unsigned long long bits;
+    memcpy(&bits, &v, sizeof(bits));
+    if (v != v) bits = 0x7ff8000000000000ull;
+#ifdef DB_EMU
+    if (bits > *out) *out = bits;
+#else
+    atomicMax(out, bits);
+#endif
+}
+
 __global__ void k_absmax(const double* __restrict__ x, int64_t count, unsigned long long* __restrict__ out)
 {
     DB_SMEM(double, red);
     double m = 0.0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
         double v = fabs(x[i]);
-        m = (v > m) ? v : m;
+        m = (v > m || v != v) ? v : m;           // a NaN wins and stays
     }
     red[threadIdx.x] = m;
     __syncthreads();
     for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-        if ((int)threadIdx.x < s) { double o = red[threadIdx.x + s]; if (o > red[threadIdx.x]) red[threadIdx.x] = o; }
+        if ((int)threadIdx.x < s) { double o = red[threadIdx.x + s]; if (o > red[threadIdx.x] || o != o) red[threadIdx.x] = o; }
         __syncthreads();
     }
     if (threadIdx.x == 0) {
         // non-negative doubles order like their bit patterns
-        unsigned long long bits;
-        double v = red[0];
-        memcpy(&bits, &v, sizeof(bits));
-#ifdef DB_EMU
-        if (bits > *out) *out = bits;
-#else
-        atomicMax(out, bits);
-#endif
+        db_publish_max(out, red[0]);
     }
 }
 
@@ -105,22 +113,16 @@ __global__ void k_cfl_max(CflArgs a, unsigned long long* __restrict__ out)
         const int64_t ix[3] = {i0, i1, i2};
         double f = 0.0;
         for (int c = 0; c < a.ncomp; ++c) f += fabs(a.u[c][e]) * a.idx[c][ix[3 - a.ncomp + c]];
-        m = (f > m) ? f : m;
+        m = (f > m || f != f) ? f : m;
     }
     red[threadIdx.x] = m;
     __syncthreads();
     for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-        if ((int)threadIdx.x < s) { double o = red[threadIdx.x + s]; if (o > red[threadIdx.x]) red[threadIdx.x] = o; }
+        if ((int)threadIdx.x < s) { double o = red[threadIdx.x + s]; if (o > red[threadIdx.x] || o != o) red[threadIdx.x] = o; }
         __syncthreads();
     }
     if (threadIdx.x == 0) {
-        unsigned long long bits; double v = red[0];
-        memcpy(&bits, &v, sizeof(bits));
-#ifdef DB_EMU
-        if (bits > *out) *out = bits;
-#else
-        atomicMax(out, bits);
-#endif
+        db_publish_max(out, red[0]);
     }
 }
 
@@ -152,22 +154,16 @@ __global__ void k_cfl_max_spherical(const double* __restrict__ up, const double*
         const int64_t ir = e % n_r;
         double f = sqrt(up[e] * up[e] + ut[e] * ut[e]) * inv_h[ir];
         if (ur) f += fabs(ur[e]) * inv_dr[ir];
-        m = (f > m) ? f : m;
+        m = (f > m || f != f) ? f : m;
     }
     red[threadIdx.x] = m;
     __syncthreads();
     for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-        if ((int)threadIdx.x < s) { double o = red[threadIdx.x + s]; if (o > red[threadIdx.x]) red[threadIdx.x] = o; }
+        if ((int)threadIdx.x < s) { double o = red[threadIdx.x + s]; if (o > red[threadIdx.x] || o != o) red[threadIdx.x] = o; }
         __syncthreads();
     }
     if (threadIdx.x == 0) {
-        unsigned long long bits; double v = red[0];
-        memcpy(&bits, &v, sizeof(bits));
-#ifdef DB_EMU
-        if (bits > *out) *out = bits;
-#else
-        atomicMax(out, bits);
-#endif
+        db_publish_max(out, red[0]);
     }
 }
 

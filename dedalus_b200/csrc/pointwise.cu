@@ -306,22 +306,16 @@ k_mmt(const double* __restrict__ mat, int m, int n, const double* __restrict__ i
 //   C fragment: lane t holds out[m0 + t/4][r0 + 2 (t%4) + {0, 1}]
 // Requirements of this path: n and inner even, 16-byte aligned pointers (else the FMA-pipe kernel above runs).
 // ---------------------------------------------------------------------------------------------------------
-#ifndef DB_EMU
 #define DM_BM 64
 #define DM_BN 64
 #define DM_BK 16
 #define DM_AS (DM_BK + 4)
 #define DM_BS (DM_BN + 4)
-__device__ __forceinline__ void db_cp_async16_zfill(void* dst, const void* src, bool valid)
-{
-    const unsigned sz = valid ? 16u : 0u;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src), "r"(sz) : "memory");
-}
 __global__ void __launch_bounds__(128)
 k_mmt_dmma(const double* __restrict__ mat, int m, int n, const double* __restrict__ in, double* __restrict__ out, int64_t inner)
 {
-    __shared__ __align__(16) double As[2][DM_BM * DM_AS];
-    __shared__ __align__(16) double Bs[2][DM_BK * DM_BS];
+    DB_SHARED_ARRAY(double, As, [2][DM_BM * DM_AS]);
+    DB_SHARED_ARRAY(double, Bs, [2][DM_BK * DM_BS]);
     const int64_t o = blockIdx.z;
     const int i0 = blockIdx.y * DM_BM;
     const int64_t r0 = (int64_t)blockIdx.x * DM_BN;
@@ -370,8 +364,7 @@ k_mmt_dmma(const double* __restrict__ mat, int m, int n, const double* __restric
             for (int a = 0; a < 4; ++a)
 #pragma unroll
                 for (int b = 0; b < 4; ++b)
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                                 : "+d"(acc[a][b][0]), "+d"(acc[a][b][1]) : "d"(af[a]), "d"(bf[b]));
+                    db_dmma_m8n8k4(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
         }
         __syncthreads();
     }
@@ -387,22 +380,23 @@ k_mmt_dmma(const double* __restrict__ mat, int m, int n, const double* __restric
         }
     }
 }
-#endif
+
+static long long g_mmt_dmma_launches = 0;
+extern "C" long long db_mmt_dmma_launches(void) { return g_mmt_dmma_launches; }
 
 extern "C" int db_mmt_apply(const double* mat, int32_t m, int32_t n, const double* in, double* out, int64_t outer, int64_t inner, void* stream)
 {
     if (outer <= 0 || inner <= 0 || m <= 0 || n <= 0) return 0;
     if (outer > 65535) { db_set_error("mmt_apply: outer too large (%lld)", (long long)outer); return 1; }
-#ifndef DB_EMU
     static int dmma = -1;
     if (dmma < 0) { const char* e = getenv("DB_MMT_DMMA"); dmma = (e && atoi(e) == 0) ? 0 : 1; }
     const bool aligned = (((uintptr_t)mat | (uintptr_t)in | (uintptr_t)out) & 15) == 0;
     if (dmma && aligned && n % 2 == 0 && inner % 2 == 0) {
         dim3 grid((unsigned)((inner + DM_BN - 1) / DM_BN), (unsigned)((m + DM_BM - 1) / DM_BM), (unsigned)outer);
         DB_LAUNCH(k_mmt_dmma, grid, dim3(128), 0, stream, mat, m, n, in, out, inner);
+        ++g_mmt_dmma_launches;
         return db_check_launch("mmt_apply(dmma)");
     }
-#endif
     dim3 grid((unsigned)((inner + MM_BN - 1) / MM_BN), (unsigned)((m + MM_BM - 1) / MM_BM), (unsigned)outer);
     DB_LAUNCH(k_mmt, grid, dim3(256), (MM_BK * MM_BM + MM_BK * MM_BN) * sizeof(double), stream, mat, m, n, in, out, outer, inner);
     return db_check_launch("mmt_apply");

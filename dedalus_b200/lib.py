@@ -91,6 +91,7 @@ SIGNATURES = {
     "db_cheb_backward_scan": (C.c_int, [PFFT, vp, vp, i64, i32, vp, i32, vp, vp]),
     "db_band_lines": (C.c_int, [vp, vp, i64, i32, vp, i32, vp, i32, i32, vp]),
     "db_mmt_apply": (C.c_int, [vp, i32, i32, vp, vp, i64, i64, vp]),
+    "db_mmt_dmma_launches": (C.c_longlong, []),
     "db_ragged_matvec": (C.c_int, [vp, vp, i32, i32, vp, vp, i64, i32, i32, i32, i32, i64, vp]),
     "db_pointwise": (C.c_int, [vp, vp, i64, i32, i32, vp, vp, vp, vp, i32, vp]),
     "db_pointwise_pairs": (C.c_int, [vp, vp, i64, i32, i32, vp, vp, vp]),

@@ -118,6 +118,9 @@ int db_band_lines(const double* in, double* out, int64_t lines, int32_t n,
 /* Dense matrix transform along an axis: out(o, i, r) = sum_j mat[i][j] * in(o, j, r).
  * Replaces SeparableMatrixTransform -> apply_dense (core/transforms.py:54-75, tools/array.py:104-129). */
 int db_mmt_apply(const double* mat, int32_t m, int32_t n, const double* in, double* out, int64_t outer, int64_t inner, void* stream);
+/* diagnostic: number of db_mmt_apply calls served by the FP64 tensor-core kernel so far (n and inner even, mat / in / out 16-byte
+ * aligned, DB_MMT_DMMA not 0); every other call runs the FMA-pipe kernel */
+long long db_mmt_dmma_launches(void);
 
 /* Ragged batch of dense matrix-vector products: the spin-weighted spherical harmonic colatitude transform.
  * Replaces SWSHColatitudeTransform.forward_reduced / backward_reduced (core/transforms.py:1263-1290): for every local
@@ -399,7 +402,10 @@ typedef struct { double re, im; int64_t sym_off; int32_t src; int32_t pad; } db_
 int db_pair_lincomb(const double* in, double* out, int64_t npair, int64_t ncol, int32_t n_out,
                     const int32_t* term_ptr, const db_pair_lin_term* terms, const double* syms, int64_t sym_div, void* stream);
 
-/* max |x| reduction (CFL / flow properties; extras/flow_tools.py:33-37 before the Allreduce) */
+/* max |x| reduction (CFL / flow properties; extras/flow_tools.py:33-37 before the Allreduce).
+ * The three reductions below ACCUMULATE: out = max(out, maximum over the input), so `out` is zero-initialised before the first call
+ * and may be passed on from one field to the next; a value already larger stays.  A NaN anywhere in the input (or already in
+ * `out`) gives NaN, as np.max does, and an infinite value gives +inf: a field that has blown up never yields a finite maximum. */
 int db_absmax(const double* x, int64_t count, double* out, void* stream);
 
 /* Advective CFL frequency: out = max over grid points of sum_i |u_i| * inv_dx_i[index along axis i]

@@ -99,7 +99,11 @@ double emu_shfl_exchange(double v, int src_lane) {
 // committed before it); cp.async.wait_group n lands, in issue order, the copies of every group but the n most recent.  The source is
 // read at landing time too: the kernels never write what they prefetch while the copy is in flight.
 namespace {
-struct CpCopy { void* dst; const void* src; size_t bytes; size_t group; };
+struct CpCopy { void* dst; const void* src; size_t bytes, src_bytes; size_t group; };       // src_bytes < bytes: the rest is zero-filled
+void cp_land(void* dst, const void* src, size_t bytes, size_t src_bytes) {
+    if (src_bytes) std::memcpy(dst, src, src_bytes);
+    std::memset((unsigned char*)dst + src_bytes, 0, bytes - src_bytes);
+}
 struct CpQueue {
     std::vector<CpCopy> copies;
     size_t head = 0, committed = 0;
@@ -122,11 +126,13 @@ CpQueue& cp_queue() {
 }
 }  // namespace
 
-void emu_cp_async(void* dst, const void* src, size_t bytes) {
-    if (!cp_late()) { std::memcpy(dst, src, bytes); return; }
+void emu_cp_async_zfill(void* dst, const void* src, size_t bytes, size_t src_bytes) {
+    if (!cp_late()) { cp_land(dst, src, bytes, src_bytes); return; }
     CpQueue& q = cp_queue();
-    q.copies.push_back({dst, src, bytes, q.committed});
+    q.copies.push_back({dst, src, bytes, src_bytes, q.committed});
 }
+
+void emu_cp_async(void* dst, const void* src, size_t bytes) { emu_cp_async_zfill(dst, src, bytes, bytes); }
 
 void emu_cp_commit() { ++cp_queue().committed; }
 
@@ -136,9 +142,17 @@ void emu_cp_wait(int n) {
     const size_t retire = q.committed - (size_t)n;        // groups 0 .. retire - 1 complete
     while (q.head < q.copies.size() && q.copies[q.head].group < retire) {
         const CpCopy& c = q.copies[q.head++];
-        std::memcpy(c.dst, c.src, c.bytes);
+        cp_land(c.dst, c.src, c.bytes, c.src_bytes);
     }
     if (q.head == q.copies.size()) { q.copies.clear(); q.head = 0; }
+}
+
+// static shared arrays poisoned so far by the running block
+static thread_local std::vector<void*> static_smem_seen;
+void emu_static_smem(void* p, size_t bytes) {
+    for (void* q : static_smem_seen) if (q == p) return;
+    static_smem_seen.push_back(p);
+    std::memset(p, 0xA5, bytes);
 }
 
 // mbarriers and bulk copies.  Copies queued under DB_EMU_BULK=late, in issue order; a wait on a barrier lands that barrier's copies.
@@ -262,6 +276,7 @@ void emu_launch(dim3 grid, dim3 block, size_t smem, const char* name, const std:
         // copies still pending when a thread of the previous block exited never land in this block's shared memory
         for (size_t t = 0; t < nthreads; ++t) cp_queues[t].reset();
         bulk_queue.clear();
+        static_smem_seen.clear();
         size_t i = 0;
         for (unsigned tz = 0; tz < block.z; ++tz)
         for (unsigned ty = 0; ty < block.y; ++ty)

@@ -71,8 +71,15 @@ static inline int atomicOr(int* p, int v) { int o = *p; *p |= v; return o; }
 // default) a copy lands only when a wait retires its group, so shared memory read before that still holds the 0xA5 poison (or an
 // older value); with DB_EMU_CP=early it lands at issue, so a slot refilled while other code still reads it shows the new value.
 void emu_cp_async(void* dst, const void* src, size_t bytes);
+// the zero-filling form (cp.async ..., cp-size, src-size): src_bytes <= bytes are copied and the rest of dst is set to zero, when the
+// copy lands; with src_bytes == 0 the source is not read at all
+void emu_cp_async_zfill(void* dst, const void* src, size_t bytes, size_t src_bytes);
 void emu_cp_commit();                // close the open group (also when it is empty), as cp.async.commit_group
 void emu_cp_wait(int n);             // land every committed group except the n most recent, as cp.async.wait_group n
+
+// a statically sized __shared__ array (DB_SHARED_ARRAY): one host array shared by the fibers; the first thread of every block to reach
+// the declaration poisons it, as emu_launch poisons the dynamic shared memory
+void emu_static_smem(void* p, size_t bytes);
 
 // mbarriers and 1-D bulk copies (cp.async.bulk ... mbarrier::complete_tx::bytes).  A barrier is one 64-bit word: low 32 bits = bytes
 // still expected in the current phase (or, for an arrival-count barrier, pending arrivals and arrivals per phase), high 32 bits =
