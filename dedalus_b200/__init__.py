@@ -11,7 +11,8 @@ from .shell import ShellBasis
 from .field import Field
 from .operators import (Differentiate, Gradient, Divergence, Laplacian, Trace, TransposeComponents,
                         Interpolate, Integrate, Lift, Convert, TimeDerivative, DotProduct, Multiply, Skew, MulCosine, Curl, curl,
-                        grad, div, lap, skew, trace, transpose, integ, ave, dot, interp, Average, UnaryGridFunction)
+                        grad, div, lap, skew, trace, transpose, integ, ave, dot, interp, Average, UnaryGridFunction,
+                        RadialComponent, AngularComponent, radial, angular)
 from .problems import IVP, LBVP
 InitialValueProblem = IVP
 LinearBoundaryValueProblem = LBVP

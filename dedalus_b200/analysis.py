@@ -8,8 +8,8 @@ Reference: Future.evaluate (core/future.py:149-206) walking the tree with the la
   * sums that contain such a term meet their operands on the grid: the conversions the reference inserts between different
     radial bases (arithmetic.py:94-98) are plain copies in grid space (operators.py:1628-1638), so nothing is truncated;
   * linear operators act on coefficients: shell gradient (dedalus_b200/shell_ivp.py ShellGradient), the separable sphere
-    operators (dedalus_b200/sphere.py evaluate_linear_expression), radial interpolation of a scalar (ShellRadialInterpolate,
-    core/basis.py:5823-5889);
+    operators (dedalus_b200/sphere.py evaluate_linear_expression), radial interpolation of scalars and tensors
+    (ShellRadialInterpolate, core/basis.py:5823-5889), radial / angular components as slices (core/basis.py:5892-5970);
   * azimuthal interpolation acts on grid values and returns a field locked to the grid (InterpolateAzimuth, basis.py:5578-5635).
 Transforms are the library's own kernels (field layout changes); the elementwise arithmetic between whole grids is done with
 torch tensor expressions on the device -- cadence-scheduled output, never part of the time step."""
@@ -159,13 +159,15 @@ class CurvilinearEvaluation:
         nonlinear_top = isinstance(e, _NONLINEAR) or (isinstance(e, (ops.Add, ops.ScalarMul)) and self._has_nonlinear(e))
         if nonlinear_top:
             return self._materialize(e, self.grid(e))
+        if isinstance(e, ops.Component):
+            return self._component(self.field(e.args[0]), e)
         shell = shell_basis_of(e.args[0]) if getattr(e, 'args', None) else None
         if isinstance(e, ops.Interpolate) and self._azimuthal(e):
             raise NotImplementedError("azimuthal interpolation returns grid data only; use it as the outermost operator of a task")
         if shell is not None:
             if isinstance(e, ops.Gradient) and shell.k == 0 and isinstance(e.args[0], Field):
                 return self._shell_gradient(self.field(e.args[0]), e)          # the kernel path (also used inside time steps)
-            if isinstance(e, ops.Interpolate) and e.axis == self.dist.get_basis_axis(shell) + 2 and not e.tensorsig:
+            if isinstance(e, ops.Interpolate) and e.axis == self.dist.get_basis_axis(shell) + 2:
                 return self._shell_radial_interpolation(self.field(e.args[0]), e)
             if isinstance(e, (ops.Gradient, ops.Divergence, ops.Laplacian, ops.Trace, ops.TransposeComponents, ops.Add, ops.ScalarMul)):
                 return self._shell_linear(e)
@@ -225,20 +227,41 @@ class CurvilinearEvaluation:
         return res
 
     def _shell_radial_interpolation(self, f, e):
-        """Scalar field at radius r0: sum_n c[m, l, n] (dR / r0)^k P_n^(alpha + k)(z(r0))  (reference basis.py:5823-5889)."""
+        """Field at radius r0: sum_n c[a, m, l, n] (dR / r0)^k P_n^(alpha + k)(z(r0)) for every regularity component a, then --
+        tensors -- the regularity -> spin recombination Q(l) of the shell chain, which leaves the spin components a field on the
+        sphere holds (reference basis.py:5823-5889)."""
         import torch
         from .shell import shell_basis_of
         from .shell_ivp import RadialOps
-        if f.tensorsig:
-            raise NotImplementedError("radial interpolation of tensor fields in output expressions")
         basis = shell_basis_of(f)
+        rank = len(f.tensorsig)
         rops = RadialOps(basis.shape[2], basis.radii, basis.alpha)
         f.change_layout('c')
         c = f.device_data()
         vec = torch.from_numpy(np.ascontiguousarray(rops.basis_functions(basis.k, e.position)[0])).to(c.device)
-        out = (c * vec).sum(dim=-1, keepdim=True)
+        out = (c * vec).sum(dim=-1, keepdim=True).contiguous()
+        if rank:
+            Nc0, Nc1 = out.shape[rank:rank + 2]
+            spin = torch.empty_like(out)
+            basis.regularity_table(rank, False, c.device, self.dist).apply(out, spin, Nc0 // 2, Nc1, sym_div=1)
+            out = spin
         res = _temp_field(e, (basis.S2_basis(radius=e.position),))
-        res.set_device_data(out.contiguous(), 'c')
+        res.set_device_data(out, 'c', scales=self.dist.remedy_scales(tuple(basis.dealias)))      # reference: outputs at the dealias scales
+        return res
+
+    def _component(self, f, e):
+        """Radial / angular component of a field on a sphere: a slice along the selected tensor axis of its data in either layout
+        -- index 2 (spin 0, or the r coordinate) and indices 0:2 (spins -, +, or the phi, theta coordinates) -- on the device
+        (reference S2RadialComponent / S2AngularComponent.operate, core/basis.py:5920-5970)."""
+        from .sphere import sphere_basis_of
+        from .shell import shell_basis_of
+        basis = sphere_basis_of(f)
+        if basis is None or shell_basis_of(f) is not None:
+            raise NotImplementedError("radial / angular components of fields on a sphere (interpolate shell fields first)")
+        d = f.device_data()
+        d = d.select(e.index, 2) if isinstance(e, ops.RadialComponent) else d.narrow(e.index, 0, 2)
+        res = _temp_field(e, (basis,))
+        res.set_device_data(d.contiguous(), f.layout, scales=f.scales)
         return res
 
     def _shell_linear(self, e):
@@ -327,6 +350,55 @@ def evaluate_curvilinear(expr):
     return CurvilinearEvaluation(expr.dist).evaluate(expr)
 
 
+def is_shell_boundary(eq):
+    """An equation of a shell problem that lives on a sphere: angular bases, none along the radius."""
+    return eq['bases'][-1] is None and eq['bases'][0] is not None
+
+
+class BoundaryData:
+    """Field right-hand side of an equation on a sphere of a shell problem (boundary data such as `angular(u(r=Ri)) = uw`,
+    `b(r=Ro) = bt`; reference: F evaluated with the other right-hand sides every stage, core/problems.py:84-100).  Each write
+    reads the expression's fields afresh, so data the user changes between steps takes effect.  The equation rows hold the spin
+    components of the sphere's coefficient packing, which is what a sphere field holds in coefficient space: a plain field is
+    copied as it is, any other expression (products, grid functions) is formed on the grid and transformed once."""
+
+    def __init__(self, solver, ie, rhs, evaluation):
+        from .shell import shell_basis_of
+        from .sphere import sphere_basis_of
+        eq = solver.problem.equations[ie]
+        ts = eq['tensorsig']
+        if len({type(cs) for cs in ts}) > 1 and not isinstance(rhs, Field):
+            raise NotImplementedError("grid expressions as data of equations with mixed spherical / S2 indices")
+        basis = sphere_basis_of(rhs)
+        shell = shell_basis_of(eq['LHS'])
+        if basis is None or any(b is not None and b is not basis for b in rhs.bases) or basis.shape != shell.shape[:2]:
+            raise NotImplementedError("boundary data must live on a sphere of the shell's angular resolution")
+        self.solver, self.rhs, self.eval, self.basis = solver, rhs, evaluation, basis
+        self.off = solver.eq_arena.offsets[ie]
+        tsh, shp = solver.eq_arena.shapes[ie]
+        self.shape = (max(int(np.prod(tsh, dtype=int)), 1),) + tuple(shp)
+        self.rank = len(ts)
+        self.spins = [int(s) for s in basis.spin_weights(ts).reshape(-1)] or [0]
+        self.cs = type(ts[0]) if ts else None
+
+    def write(self, eq_t):
+        from .sphere import grid_to_components
+        from .coords import S2Coordinates
+        n = int(np.prod(self.shape))
+        dst = eq_t[self.off:self.off + n].view(self.shape)
+        if isinstance(self.rhs, Field):
+            self.rhs.change_layout('c')
+            dst.copy_(self.rhs.device_data().reshape(self.shape))
+            return
+        g = self.eval.grid(self.rhs)
+        sl = [self.solver.dist.grid_local_slice(ax, self.basis, self.basis.dealias[ax]) for ax in range(2)]
+        full = (self.shape[0], sl[0].stop - sl[0].start, sl[1].stop - sl[1].start)
+        tsh = tuple(g.shape[:self.rank])
+        g = g.reshape(tsh + tuple(g.shape[self.rank:self.rank + 2])).expand(tsh + full[1:]).reshape(full).contiguous()
+        c = grid_to_components(self.basis, g, self.spins, self.rank, cs=self.cs or S2Coordinates, dist=self.solver.dist)
+        dst.copy_(c.reshape(self.shape))
+
+
 class GenericCurvilinearRHS:
     """Right-hand sides of sphere / shell problems that the fused plans (sphere.SphereRHSPlan, shell_ivp.ShellRHSPlan) do not cover --
     grid functions, forcings, fields that are not problem variables, products with radial profiles, operators applied to products:
@@ -340,6 +412,7 @@ class GenericCurvilinearRHS:
         self.dist = solver.dist
         self.eval = CurvilinearEvaluation(solver.dist)
         self.entries = []                 # (equation index, expression, conversion matrix on the device or None)
+        self.boundary = []                # BoundaryData of the equations on a sphere of a shell
         self.static = []
         problem = solver.problem
         for ie, eq in enumerate(problem.equations):
@@ -349,7 +422,10 @@ class GenericCurvilinearRHS:
                     self._constant(ie, eq, float(rhs))
                 continue
             if any(b is None for b in eq['bases']):
-                raise NotImplementedError("field right-hand sides of lower-dimensional equations on curvilinear domains")
+                if not (solver.shell and is_shell_boundary(eq)):
+                    raise NotImplementedError("field right-hand sides of lower-dimensional equations on curvilinear domains")
+                self.boundary.append(BoundaryData(solver, ie, rhs, self.eval))
+                continue
             self.entries.append([ie, rhs, None, shell_basis_of(eq['LHS'])])
 
     def _constant(self, ie, eq, value):
@@ -379,6 +455,8 @@ class GenericCurvilinearRHS:
         import torch
         from .sphere import sphere_basis_of
         arena = self.solver.eq_arena
+        for bd in self.boundary:
+            bd.write(eq_t)
         for ie, rhs, _, eq_shell in self.entries:
             # F on the dealiased grid, then ONE forward transform in the equation's own basis: the reference converts F to the
             # equation's bases while it is on the grid (a copy), so no intermediate truncation in the expression's basis happens

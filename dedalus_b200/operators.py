@@ -398,6 +398,39 @@ class Lift(LinearOperator):
         self.bases = tuple(b)
 
 
+class Component(LinearOperator):
+    """Selection along one tensor index over SphericalCoordinates (reference Component, core/operators.py:2190-2226): on a sphere
+    basis the spin components (-, +, 0) of that index; radial = spin 0, angular = spins (-, +) (core/basis.py:5892-5970)."""
+    def __init__(self, A, index=0):
+        if not isinstance(A, Operand):
+            raise ValueError("Component selection needs an operand.")
+        rank = len(A.tensorsig)
+        if index < 0:
+            index += rank
+        if not 0 <= index < rank:
+            raise ValueError("index greater than rank")
+        self.args = [A]
+        self.index = index
+        self.coordsys = A.tensorsig[index]
+        if getattr(self.coordsys, 'S2coordsys', None) is None:
+            raise NotImplementedError("radial / angular components of indices over SphericalCoordinates only")
+        self.dist, self.dtype, self.bases = A.dist, A.dtype, A.bases
+
+
+class RadialComponent(Component):
+    def __init__(self, A, index=0):
+        super().__init__(A, index)
+        ts = A.tensorsig
+        self.tensorsig = ts[:self.index] + ts[self.index + 1:]
+
+
+class AngularComponent(Component):
+    def __init__(self, A, index=0):
+        super().__init__(A, index)
+        ts = A.tensorsig
+        self.tensorsig = ts[:self.index] + (self.coordsys.S2coordsys,) + ts[self.index + 1:]
+
+
 class Convert(LinearOperator):
     """Convert(A, bases): per-axis tuple of output bases, or -- the reference's form (core/operators.py:1533-1560) -- ONE output
     basis, which replaces the operand's basis along that basis' axis."""
@@ -427,6 +460,8 @@ def ave(A, coords=None): return Integrate(A, coords, average=True)
 def Average(A, coords=None): return Integrate(A, coords, average=True)
 def dot(A, B): return DotProduct(A, B)
 def interp(A, **positions): return A(**positions)
+def radial(A, index=0): return RadialComponent(A, index)
+def angular(A, index=0): return AngularComponent(A, index)
 
 
 # --------------------------------------------------------------------------------------------------------

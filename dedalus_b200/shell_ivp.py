@@ -312,6 +312,14 @@ class ShellLowering:
                     return []
                 return [(s, Q[s, co] * (row @ B)) for s in range(Q.shape[0]) if Q[s, co] != 0]
             return _map(n, fn, kind='sphere', k=0, nrad=1)
+        if isinstance(e, ops.Component):
+            # a selection of spin components (reference S2RadialComponent / S2AngularComponent.subproblem_matrix,
+            # core/basis.py:5892-5970): the blocks move to the component they land on, unchanged
+            n = self.lower(e.args[0], ell)
+            if n.kind != 'sphere':
+                raise NotImplementedError("radial / angular components on a shell: of fields on a sphere (interpolate first)")
+            sel = component_selection(e)
+            return _map(n, lambda co, B: [(sel[co], B)] if co in sel else [], rank=len(e.tensorsig))
         if isinstance(e, ops.Integrate):
             n = self.lower(e.args[0], ell)
             if n.kind != 'shell' or n.rank != 0 or e.average:
@@ -351,19 +359,40 @@ def _clean(M, tol=1e-13):
     return M
 
 
+def component_selection(e):
+    """{operand component: result component} of a radial / angular component (C order over the tensor dims): the radial one keeps
+    the components whose selected index is the spin-0 one (index 2) and drops that index; the angular one keeps those with spin
+    -, + (indices 0, 1) at the same positions, the index now running over the 2 components of the S2 coordinates."""
+    dims_in = tuple(cs.dim for cs in e.args[0].tensorsig)
+    dims_out = tuple(cs.dim for cs in e.tensorsig)
+    radial = isinstance(e, ops.RadialComponent)
+    sel = {}
+    for c, idx in enumerate(np.ndindex(*dims_in)):
+        a = idx[e.index]
+        if radial and a == 2:
+            out = idx[:e.index] + idx[e.index + 1:]
+        elif not radial and a < 2:
+            out = idx
+        else:
+            continue
+        sel[c] = int(np.ravel_multi_index(out, dims_out)) if dims_out else 0
+    return sel
+
+
 def component_layout(items, basis, ell):
-    """Natural ordering of the unknowns (or equation rows) of degree l: for each item (kind, rank), its components, each with its
-    radial size, and their validity (reference: regularity_allowed / |s| <= l / l == 0)."""
+    """Natural ordering of the unknowns (or equation rows) of degree l: for each item (kind, tensor signature), its components, each
+    with its radial size, and their validity (reference: regularity_allowed / |total spin| <= l / l == 0).  Fields on a sphere
+    may carry S2 indices (2 spin components -, +) next to spherical ones (3: -, +, 0)."""
     Nr = basis.shape[2]
     out = []
-    for it, (kind, rank) in enumerate(items):
-        ncomp = 3 ** rank
-        for c in range(ncomp):
-            idx = tuple(np.unravel_index(c, (3,) * rank)) if rank else ()
+    for it, (kind, tensorsig) in enumerate(items):
+        for c, idx in enumerate(np.ndindex(*(cs.dim for cs in tensorsig))):
             if kind == 'shell':
+                if any(cs.dim != 3 for cs in tensorsig):
+                    raise NotImplementedError("S2 tensor indices of shell fields")
                 valid, n = regularity_allowed(ell, idx), Nr
             elif kind == 'sphere':
-                valid, n = abs(sum(REG[i] for i in idx)) <= ell, 1
+                valid, n = abs(sum(cs.spin_ordering[i] for cs, i in zip(tensorsig, idx))) <= ell, 1
             else:
                 valid, n = (ell == 0), 1
             out.append(dict(item=it, comp=c, n=n, valid=valid))
@@ -374,12 +403,12 @@ def assemble(low, ell):
     """(M, L, row layout, column layout) of degree l in natural ordering: dense arrays over ALL components (invalid ones
     included, as zero rows / columns)."""
     problem = low.problem
-    var_items = [(low.kind_of(v)[0], len(v.tensorsig)) for v in low.variables]
+    var_items = [(low.kind_of(v)[0], v.tensorsig) for v in low.variables]
     cols = component_layout(var_items, low.basis, ell)
     col_off = np.cumsum([0] + [c['n'] for c in cols])
     col_index = {(c['item'], c['comp']): i for i, c in enumerate(cols)}
     eq_nodes = [low.lower(eq['LHS'], ell) for eq in problem.equations]
-    eq_items = [(low.kind_of(eq['LHS'])[0], len(eq['tensorsig'])) for eq in problem.equations]
+    eq_items = [(low.kind_of(eq['LHS'])[0], eq['tensorsig']) for eq in problem.equations]
     rows = component_layout(eq_items, low.basis, ell)
     row_off = np.cumsum([0] + [r['n'] for r in rows])
     row_index = {(r['item'], r['comp']): i for i, r in enumerate(rows)}
@@ -443,8 +472,8 @@ class ShellSystems:
         arr = (DenseSys * self.nsys)()
         vec_off, xi_all, fi_all = 0, [], []
         mode = {m: sb.mode_columns(m) for m in range(Nphi // 2)}
-        var_items = [(low.kind_of(v)[0], len(v.tensorsig)) for v in low.variables]
-        eq_items = [(low.kind_of(eq['LHS'])[0], len(eq['tensorsig'])) for eq in problem.equations]
+        var_items = [(low.kind_of(v)[0], v.tensorsig) for v in low.variables]
+        eq_items = [(low.kind_of(eq['LHS'])[0], eq['tensorsig']) for eq in problem.equations]
         self.total_modes = 0
         for ell, p in enumerate(per_l):
             ms_l = [m for m in local_ms if m <= ell and mode[m][0] is not None]       # this rank's columns of degree l
@@ -643,10 +672,12 @@ class ShellRHSPlan:
       2. every operand to the grid (dedalus_b200/shell.py shell_components_to_grid), one pointwise launch for all products
       3. products back to coefficients in the product basis k = k_A + k_B, converted to the equation's basis with E^dk and
          written into the equation arena (db_mmt_apply with -E^dk folded in).
-    Supported: sums of numeric multiples of dot / tensor products whose factors are state fields or gradients of state fields."""
+    Supported: sums of numeric multiples of dot / tensor products whose factors are state fields or gradients of state fields; the
+    equations on a sphere (boundary conditions) take field data, written every stage by analysis.BoundaryData."""
 
     def __init__(self, solver):
         import torch
+        from .analysis import BoundaryData, CurvilinearEvaluation, is_shell_boundary
         self.solver = solver
         problem = solver.problem
         dev = self.device = solver.device
@@ -704,11 +735,15 @@ class ShellRHSPlan:
             return {c: [(1.0, (o['g0'] + c,))] for c in range(n)}, o['k'], n
 
         self.products = []            # (eq index, rank, k of the product basis, terms per component)
+        self.boundary = []            # data of the equations on a sphere (analysis.BoundaryData)
         for ie, eq in enumerate(problem.equations):
             rhs = eq['RHS']
             if not isinstance(rhs, ops.Operand):
                 if rhs != 0:
                     self._add_constant(ie, eq, float(rhs), low)
+                continue
+            if is_shell_boundary(eq):
+                self.boundary.append(BoundaryData(solver, ie, rhs, CurvilinearEvaluation(dist)))
                 continue
             terms = rhs.args if isinstance(rhs, ops.Add) else [rhs]
             acc, kprod, ncomp = None, None, None
@@ -788,6 +823,8 @@ class ShellRHSPlan:
         from .lib import get_lib, current_stream
         from .shell import shell_components_to_grid, shell_grid_to_components
         from .solvers import Timed
+        for bd in self.boundary:
+            bd.write(eq_t)
         if self.n_p == 0:
             return
         solver, basis = self.solver, self.basis

@@ -256,10 +256,14 @@ class SphereBasis(Basis):
         return self._plans[key]
 
     def recombination_table(self, rank, forward, device, cs=S2Coordinates):
-        """Device program of db_pair_lincomb for the component <-> spin recombination of a rank-`rank` tensor over `cs`."""
-        key = ('rec', rank, bool(forward), str(device), cs.dim)
+        """Device program of db_pair_lincomb for the component <-> spin recombination of a rank-`rank` tensor over `cs` (one
+        coordinate-system class for every index, or a tuple of them: spherical and S2 indices mixed)."""
+        css = tuple(cs) if isinstance(cs, tuple) else (cs,) * rank
+        key = ('rec', bool(forward), str(device), tuple(c.dim for c in css))
         if key not in self._plans:
-            U = cs.U_forward(rank) if forward else cs.U_backward(rank)
+            U = np.ones((1, 1))
+            for c in css:
+                U = np.kron(U, c.U_forward(1) if forward else c.U_backward(1))
             self._plans[key] = PairProgram.from_matrix(U, device)
         return self._plans[key]
 
@@ -434,7 +438,7 @@ def transform_sphere_field(field, layout):
     ax = field.dist.get_basis_axis(basis)
     scales = field.scales[ax:ax + 2]
     rank = len(field.tensorsig)
-    cs = type(field.tensorsig[0]) if rank else S2Coordinates
+    cs = tuple(type(c) for c in field.tensorsig) if rank else S2Coordinates
     trail = (1,) * (field.dist.dim - ax - 2)             # a sphere inside a 3-D distributor: trailing constant axis
     spins = [int(s) for s in basis.spin_weights(field.tensorsig).reshape(-1)]
     data = field.device_data()
