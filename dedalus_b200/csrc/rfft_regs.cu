@@ -57,6 +57,19 @@ __device__ __forceinline__ double* out_row_ptr(const RegArgs& a, double* gout, i
     return gout + row_offset(o, r, rows, a.out_rpb, a.out_blk_stride, inner);
 }
 
+// The forward store's destination in the fused x pass: plain rows only.  Three scalars, so that it stays in registers; a RegArgs
+// there would go to local memory (its out_blk_ptr array is indexed at run time).
+struct PlainRows {
+    const double* twn;
+    int64_t inner;
+    int32_t M;
+};
+
+__device__ __forceinline__ double* out_row_ptr(const PlainRows&, double* gout, int64_t o, int r, int rows, int64_t inner)
+{
+    return gout + (o * rows + r) * inner;
+}
+
 __device__ __forceinline__ double2 cadd2(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ double2 csub2(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }
 
@@ -335,8 +348,9 @@ __device__ __forceinline__ void rfwd_park(const double2 (&z)[Q], double2* xch, i
 }
 
 // forward: the two real lines' cos / -sin coefficients of every mode k <= Kmax this thread owns, scaled, stored to rows 2k, 2k+1
-template <int Q, int NB, int P>
-__device__ __forceinline__ void rfwd_store(const double2 (&z)[Q], const double2* xch, int p, int r, const RegArgs& a, double* gout,
+// (Args: RegArgs or PlainRows)
+template <int Q, int NB, int P, class Args>
+__device__ __forceinline__ void rfwd_store(const double2 (&z)[Q], const double2* xch, int p, int r, const Args& a, double* gout,
                                            int64_t o)
 {
     constexpr int N = 3 * Q * NB;
@@ -372,8 +386,8 @@ struct OutCol { double* g; int64_t o; };       // a pair's column in the output 
 // the whole forward transform of the grid tile staged in `buf` ([N][P] double2), which is also its exchange buffer; every
 // thread of the CTA calls it (it contains barriers), and `buf` may be overwritten once the caller has passed a barrier after it.
 // dest() -> (this pair's column in the output rows, outer index) is evaluated only at the store.
-template <int Q, int NB, int P, class Dest>
-__device__ __forceinline__ void rfwd_tile(double2* buf, int p, int r, const RegArgs& a, Dest dest)
+template <int Q, int NB, int P, class Args, class Dest>
+__device__ __forceinline__ void rfwd_tile(double2* buf, int p, int r, const Args& a, Dest dest)
 {
     constexpr int NA = 3 * Q, H = NB / 2;
     const bool in_1 = r < 2 * NA, in_2 = r < 3 * NB;
@@ -491,7 +505,9 @@ k_rfwd_regs(RegArgs a, TileWalk tw_)
 //
 // Shared memory at n = 384, M = 256, three held factors: exchange [N][P] 48 KB + staging [M][P] 32 KB + 3 held tiles 144 KB =
 // 224 KB, one CTA of 384 threads per SM.  Holding a factor in registers instead (32 more per thread, for a second staging slot)
-// takes the kernel past the 168 registers a 384-thread CTA can have and makes it spill.
+// takes the kernel past the 168 registers a 384-thread CTA can have and makes it spill.  That shared-memory carve-out leaves the
+// SM about 30 KB of L1, so local memory is expensive here: the forward store gets a destination that stays in registers
+// (PlainRows), and the thread roles are re-derived per item (see below).
 // ---------------------------------------------------------------------------------------------------------
 #define XP_STREAM 3             // factor code of the streamed input (0..2: held factors, -1: none)
 
@@ -507,6 +523,20 @@ struct XProdArgs {
     const int32_t* loads;       // src of every item with src >= 0, in item order
     int32_t n_loads;
 };
+
+// threadIdx.x (< THREADS) read anew at every call (volatile asm), so that nothing derived from it can be hoisted out of the loop
+// it is read in; the bound keeps the compiler's knowledge of which thread roles exist
+template <int THREADS> __device__ __forceinline__ int opaque_tid()
+{
+#ifdef DB_EMU
+    return (int)threadIdx.x;
+#else
+    unsigned t;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+    __builtin_assume(t < THREADS);
+    return (int)t;
+#endif
+}
 
 // MINB: the register budget per thread (168 at n = 384) is the same at every tile height: 8 / P CTAs of 48 P threads per SM
 template <int Q, int NB, int P> struct XpGeom {
@@ -528,14 +558,8 @@ k_rfft_x_products(XProdArgs a, int64_t total)
     double2* X = sm;                                       // [N][P] exchange / forward staging
     double2* stg = X + N * P;                              // [M][P] coefficient rows of the next transform
     double2* hs = stg + M * P;                             // held factors: [H][THREADS] each, private to their thread
-    const int tid = threadIdx.x, p = threadIdx.x % P, r = threadIdx.x / P;
-    const bool in_a = r < 3 * NB, in_b = r < 2 * NA;
-    const int k1 = r % NA, h = r / NA;
     const int64_t inner = a.inner;
-    RegArgs fa;                                            // forward store: plain row addressing into the output arrays
-    fa.in = nullptr; fa.out = a.out; fa.twn = a.twn; fa.inner = inner; fa.M = M; fa.deriv = 0; fa.kscale = 0.0;
-    fa.in_rpb = 0; fa.out_rpb = 0; fa.in_blk_stride = 0; fa.out_blk_stride = 0; fa.out_peers = 0;
-    for (int i = 0; i < 8; ++i) fa.out_blk_ptr[i] = nullptr;
+    const PlainRows fa{a.twn, inner, M};
     // load sequence of this CTA: for each of its tiles, every entry of a.loads
     int64_t ld_t = blockIdx.x;
     int ld_k = 0;
@@ -553,6 +577,11 @@ k_rfft_x_products(XProdArgs a, int64_t total)
     for (int64_t t = blockIdx.x; t < total; t += gridDim.x) {
         for (int i = 0; i < a.n_items; ++i) {
             const db_xprod_item* itp = a.items + i;
+            // Thread roles per item: derived once per kernel, the shared-memory and twiddle addresses and derivative factors of
+            // every unrolled stage would be hoisted out of the loop, live across all its transforms, and spill.
+            const int tid = opaque_tid<THREADS>(), p = tid % P, r = tid / P;
+            const bool in_a = r < 3 * NB, in_b = r < 2 * NA;
+            const int k1 = r % NA, h = r / NA;
             double2 v[H];
             if (itp->src >= 0) {
                 db_cp_wait<0>();
@@ -569,7 +598,7 @@ k_rfft_x_products(XProdArgs a, int64_t total)
                 db_cp_commit();
                 if (in_b) rbwd_stage_b<Q, NB, P>(X, p, r, v);
             }
-            const db_xprod_item it = *itp;                 // (read after the transform: not live across it)
+            const db_xprod_item it = *itp;                 // (read after the transforms, and again at the store: not live across them)
             if (in_b) {
                 auto factor = [&](int f, int m) -> double2 {
                     return f == XP_STREAM ? v[m] : hs[(f * H + m) * THREADS + tid];
@@ -596,7 +625,7 @@ k_rfft_x_products(XProdArgs a, int64_t total)
                     for (int m = 0; m < H; ++m) { X[(k1 + NA * (2 * m + h)) * P + p] = acc[m]; acc[m] = make_double2(0.0, 0.0); }
                 }
                 __syncthreads();
-                rfwd_tile<Q, NB, P>(X, p, r, fa, [&] { return OutCol{a.out + it.out * a.out_stride + t * (2 * P) + 2 * p, 0}; });
+                rfwd_tile<Q, NB, P>(X, p, r, fa, [&] { return OutCol{a.out + itp->out * a.out_stride + t * (2 * P) + 2 * p, 0}; });
                 __syncthreads();
             }
         }
