@@ -603,15 +603,17 @@ __global__ void __launch_bounds__(FFT_THREADS, DIRECT ? 3 : 2) k_fft(FftArgs a)
             auto getX = [&](int k, int t) -> double2 {
                 if (KIND == K_RBWD) {
                     if (k > Kmax) return make_double2(0.0, 0.0);
+                    // odd M: the last mode has a cos slot only, its -sin part is zero (row M is not part of the line)
+                    const bool has_sin = 2 * k + 1 < M;
                     double2 z;
                     if (DIRECT) {
                         if (t >= gi.Tc) return make_double2(0.0, 0.0);
                         const int64_t o = gi.base + (int64_t)(2 * k) * gi.estride + t * gi.lstride;
                         if (k == 0) return make_double2((deriv > 0) ? 0.0 : gin[o], 0.0);
-                        z = make_double2(0.5 * gin[o], 0.5 * gin[o + gi.estride]);
+                        z = make_double2(0.5 * gin[o], has_sin ? 0.5 * gin[o + gi.estride] : 0.0);
                     } else {
                         if (k == 0) return make_double2((deriv > 0) ? 0.0 : cof[t], 0.0);
-                        z = make_double2(0.5 * cof[(2 * k) * TP + t], 0.5 * cof[(2 * k + 1) * TP + t]);
+                        z = make_double2(0.5 * cof[(2 * k) * TP + t], has_sin ? 0.5 * cof[(2 * k + 1) * TP + t] : 0.0);
                     }
                     if (deriv > 0) {
                         double f = 1.0;

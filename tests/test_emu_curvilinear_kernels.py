@@ -4,9 +4,10 @@ long-double references at their edge shapes; GPU version: tests/test_gpu_1d_curv
 tensor-core product from warp shuffles and queues the zero-filling 16-byte cp.async copies like every other cp.async, so k_mmt_dmma
 runs here as it does on the GPU, under both landing models of the copies and both thread orders."""
 import os, subprocess, sys, pathlib
-import numpy as np, pytest
+import pytest
 from emu import emu_lib as E
 import curvilinear_kernel_cases as K
+from kernel_backends import EmuArrays
 
 ROOT = pathlib.Path(__file__).resolve().parents[1]
 
@@ -18,31 +19,7 @@ def emulation():
     E.uninstall()
 
 
-class _EmuArrays:
-    """numpy arrays + the emulated library, behind the interface curvilinear_kernel_cases uses."""
-    lib = property(lambda self: E.emu())
-    stream = None
-    sms = 132                       # csrc/core.cu: db_num_sms() of the emulation
-
-    def dev(self, a):
-        return self.dev_at(a, False)
-
-    def dev_at(self, a, off):
-        a = np.ascontiguousarray(a)
-        raw = np.empty(a.nbytes + 32, dtype=np.uint8)
-        start = (-raw.ctypes.data) % 16 + (8 if off else 0)
-        out = raw[start:start + a.nbytes].view(a.dtype).reshape(a.shape)
-        out[...] = a
-        return out
-
-    def ptr(self, a):
-        return E.ptr(a)
-
-    def host(self, a):
-        return a
-
-
-B = _EmuArrays()
+B = EmuArrays()
 
 
 # ---- csrc/dense.cu

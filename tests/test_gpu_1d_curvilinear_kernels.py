@@ -2,54 +2,12 @@
 FMA pipe, ragged colatitude products, pair combinations, index moves, max reductions -- on the GPU, against long-double references at
 their edge shapes; the same bodies run through the emulation in tests/test_emu_curvilinear_kernels.py.  Here also the sizes the
 emulation leaves out: dense systems of n = 801 and 1000, past the size at which the solve keeps its columns in global memory."""
-import ctypes as C
-import numpy as np, pytest
+import pytest
 import curvilinear_kernel_cases as K
+from kernel_backends import DeviceArrays
 
 pytestmark = pytest.mark.gpu
-
-
-class _DeviceArrays:
-    """torch tensors on the compute device + the bound library, behind the interface curvilinear_kernel_cases uses."""
-
-    @property
-    def lib(self):
-        from dedalus_b200.lib import get_lib
-        return get_lib()
-
-    @property
-    def stream(self):
-        from dedalus_b200.lib import current_stream
-        return current_stream()
-
-    @property
-    def sms(self):
-        import torch
-        return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count if torch.cuda.is_available() else 132
-
-    def dev(self, a):
-        return self.dev_at(a, False)
-
-    def dev_at(self, a, off):
-        import torch
-        from dedalus_b200.lib import compute_device
-        a = np.ascontiguousarray(a)
-        raw = torch.empty(a.nbytes + 32, dtype=torch.uint8, device=compute_device())
-        start = (-raw.data_ptr()) % 16 + (8 if off else 0)
-        out = raw[start:start + a.nbytes]
-        out.copy_(torch.from_numpy(a.reshape(-1).view(np.uint8).copy()))
-        out = out.view(getattr(torch, a.dtype.name)).reshape(a.shape)
-        assert out.data_ptr() % 16 == (8 if off else 0)
-        return out
-
-    def ptr(self, t):
-        return C.c_void_p(t.data_ptr())
-
-    def host(self, t):
-        return t.cpu().numpy()
-
-
-B = _DeviceArrays()
+B = DeviceArrays()
 
 
 # ---- csrc/dense.cu
