@@ -15,6 +15,14 @@
 #define DB_SET_SMEM_ATTR(kern) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
 #endif
 
+// a 16-byte global access (double2) must be 16-byte aligned: the emulation checks the address and aborts with a message, the GPU
+// build compiles nothing
+#ifdef DB_EMU
+#define DB_CHECK_ALIGN16(p) emu_check_align16((const void*)(p), __func__)
+#else
+#define DB_CHECK_ALIGN16(p) ((void)0)
+#endif
+
 #ifdef DB_EMU
 #define DB_LDCS(p) (*(p))
 #else

@@ -8,9 +8,13 @@
 #include "db_common.cuh"
 #include <cstdlib>
 #include <cstdint>
-#include <cstdint>
 
 #define PW_TILE 256
+
+// launches per kernel so far (db_pointwise_launches): k_pointwise, k_pointwise_v3, k_pointwise_pairs, transpose 16-byte branch,
+// transpose 8-byte branch
+static long long g_pw_launches[5] = {0, 0, 0, 0, 0};
+extern "C" long long db_pointwise_launches(int32_t kind) { return kind >= 0 && kind < 5 ? g_pw_launches[kind] : -1; }
 
 __global__ void __launch_bounds__(PW_TILE)
 k_pointwise(const double* __restrict__ in, double* __restrict__ out, int64_t npoints, int n_in, int n_out,
@@ -39,38 +43,7 @@ k_pointwise(const double* __restrict__ in, double* __restrict__ out, int64_t npo
     }
 }
 
-// two points per thread, 128-bit global and shared accesses (npoints even, 16-byte aligned arrays)
-__global__ void __launch_bounds__(PW_TILE)
-k_pointwise_v2(const double* __restrict__ in, double* __restrict__ out, int64_t npoints, int n_in, int n_out,
-               const int32_t* __restrict__ term_ptr, const double* __restrict__ coef,
-               const int32_t* __restrict__ fac_ptr, const int32_t* __restrict__ fac)
-{
-    DB_SMEM(double, tile);                         // [n_in][2*PW_TILE]
-    double2* tile2 = reinterpret_cast<double2*>(tile);
-    const int64_t np2 = npoints >> 1;
-    for (int64_t q0 = (int64_t)blockIdx.x * PW_TILE; q0 < np2; q0 += (int64_t)gridDim.x * PW_TILE) {
-        const int64_t q = q0 + threadIdx.x;
-        const bool live = q < np2;
-        for (int i = 0; i < n_in; ++i)
-            tile2[i * PW_TILE + threadIdx.x] = live ? reinterpret_cast<const double2*>(in + (int64_t)i * npoints)[q] : make_double2(0.0, 0.0);
-        if (live) {
-            for (int o = 0; o < n_out; ++o) {
-                double a0 = 0.0, a1 = 0.0;
-                for (int t = term_ptr[o]; t < term_ptr[o + 1]; ++t) {
-                    double p0 = coef[t], p1 = p0;
-                    for (int f = fac_ptr[t]; f < fac_ptr[t + 1]; ++f) {
-                        const double2 v = tile2[fac[f] * PW_TILE + threadIdx.x];
-                        p0 *= v.x; p1 *= v.y;
-                    }
-                    a0 += p0; a1 += p1;
-                }
-                reinterpret_cast<double2*>(out + (int64_t)o * npoints)[q] = make_double2(a0, a1);
-            }
-        }
-    }
-}
-
-// v3: the per-thread staging of v2 with the copies made asynchronous (16-byte cp.async, L1 bypass) and double buffered:
+// v3: two points per thread, staged with 16-byte asynchronous copies (cp.async, L1 bypass), double buffered:
 // the n_in loads of the NEXT tile are in flight while the current tile's products are evaluated, and no load result
 // ever sits on a register dependency.  Each thread only reads the slots it filled itself, so no block barrier.
 #define PW3_T 128
@@ -110,6 +83,7 @@ k_pointwise_v3(const double* __restrict__ in, double* __restrict__ out, int64_t 
                     }
                     a0 += p0; a1 += p1;
                 }
+                DB_CHECK_ALIGN16(out + (int64_t)o * npoints + 2 * q);
                 reinterpret_cast<double2*>(out + (int64_t)o * npoints)[q] = make_double2(a0, a1);
             }
         }
@@ -170,6 +144,7 @@ k_pointwise_pairs(const double* __restrict__ in, double* __restrict__ out, int64
                         a0 = fma(p0, vb.x, a0); a1 = fma(p1, vb.y, a1);
                     } else { a0 += p0; a1 += p1; }
                 }
+                DB_CHECK_ALIGN16(out + (int64_t)o * npoints + 2 * q);
                 reinterpret_cast<double2*>(out + (int64_t)o * npoints)[q] = make_double2(a0, a1);
             }
         }
@@ -186,6 +161,10 @@ extern "C" int db_pointwise_pairs(const double* in, double* out, int64_t npoints
         db_set_error("pointwise_pairs: needs an even point count, 16-byte aligned arrays and at most %d inputs", (int)(DB_MAX_SMEM / (2 * PW3_T * sizeof(double2))));
         return 1;
     }
+    if (reinterpret_cast<uintptr_t>(terms) & 15) {         // read as int4 records
+        db_set_error("pointwise_pairs: the term records must be 16-byte aligned");
+        return 1;
+    }
     int per_sm = (int)((size_t)(226 * 1024) / (smem3 + 1024));
     if (per_sm > 8) per_sm = 8;
     int64_t blocks = (npoints / 2 + PW3_T - 1) / PW3_T;
@@ -199,6 +178,7 @@ extern "C" int db_pointwise_pairs(const double* in, double* out, int64_t npoints
     }
 #endif
     DB_LAUNCH(k_pointwise_pairs, dim3((unsigned)blocks), dim3(PW3_T), smem3, stream, in, out, npoints, n_in, n_out, term_ptr, terms);
+    ++g_pw_launches[2];
     return db_check_launch("pointwise_pairs");
 }
 
@@ -224,24 +204,27 @@ extern "C" int db_pointwise(const double* in, double* out, int64_t npoints, int3
         }
 #endif
         DB_LAUNCH(k_pointwise_v3, dim3((unsigned)blocks3), dim3(PW3_T), smem3, stream, in, out, npoints, n_in, n_out, term_ptr, coef, fac_ptr, fac);
+        ++g_pw_launches[1];
         return db_check_launch("pointwise");
     }
-    size_t smem = (size_t)n_in * PW_TILE * sizeof(double) * (vec ? 2 : 1);
-    if (smem > (size_t)DB_MAX_SMEM) { db_set_error("pointwise: too many inputs (%d)", n_in); return 1; }
-    const int64_t items = vec ? npoints / 2 : npoints;
-    int64_t blocks = (items + PW_TILE - 1) / PW_TILE;
+    // odd point count, a misaligned array, or more inputs than v3's two buffers hold: one point per thread, single buffered
+    const size_t smem = (size_t)n_in * PW_TILE * sizeof(double);
+    if (smem > (size_t)DB_MAX_SMEM) {
+        db_set_error("pointwise: too many inputs (%d, at most %d)", n_in, (int)(DB_MAX_SMEM / (PW_TILE * sizeof(double))));
+        return 1;
+    }
+    int64_t blocks = (npoints + PW_TILE - 1) / PW_TILE;
     const int64_t cap = (int64_t)db_num_sms() * 8;
     if (blocks > cap) blocks = cap;
 #ifndef DB_EMU
     static bool attr = false;
     if (!attr) {
         cudaFuncSetAttribute(k_pointwise, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
-        cudaFuncSetAttribute(k_pointwise_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_MAX_SMEM);
         attr = true;
     }
 #endif
-    if (vec) DB_LAUNCH(k_pointwise_v2, dim3((unsigned)blocks), dim3(PW_TILE), smem, stream, in, out, npoints, n_in, n_out, term_ptr, coef, fac_ptr, fac);
-    else DB_LAUNCH(k_pointwise, dim3((unsigned)blocks), dim3(PW_TILE), smem, stream, in, out, npoints, n_in, n_out, term_ptr, coef, fac_ptr, fac);
+    DB_LAUNCH(k_pointwise, dim3((unsigned)blocks), dim3(PW_TILE), smem, stream, in, out, npoints, n_in, n_out, term_ptr, coef, fac_ptr, fac);
+    ++g_pw_launches[0];
     return db_check_launch("pointwise");
 }
 
@@ -376,7 +359,10 @@ k_mmt_dmma(const double* __restrict__ mat, int m, int n, const double* __restric
 #pragma unroll
         for (int b = 0; b < 4; ++b) {
             const int64_t gr = r0 + wn + b * 8 + 2 * (lane & 3);
-            if (gr < inner) *reinterpret_cast<double2*>(outb + (int64_t)gi * inner + gr) = make_double2(acc[a][b][0], acc[a][b][1]);
+            if (gr < inner) {
+                DB_CHECK_ALIGN16(outb + (int64_t)gi * inner + gr);
+                *reinterpret_cast<double2*>(outb + (int64_t)gi * inner + gr) = make_double2(acc[a][b][0], acc[a][b][1]);
+            }
         }
     }
 }
@@ -475,13 +461,14 @@ extern "C" int db_ragged_matvec(const double* mats, const db_ragged_entry* entri
 // The reverse hop swaps the roles.  Blocks are assumed equal (n2 % P == 0, n1 % P == 0).
 // ---------------------------------------------------------------------------------------------------------
 // All four permutes move whole contiguous chunks: for fixed (batch b, row i, peer p) the block of `clen` doubles is
-// contiguous on both sides.  One CTA (or several, via blockIdx.y) copies one chunk with 128-bit accesses; the only
-// index arithmetic is per chunk.
+// contiguous on both sides.  One CTA (or several, via blockIdx.y) copies one chunk; the only index arithmetic is per chunk.
+// Every chunk offset below is a multiple of clen, so with clen even and both base pointers 16-byte aligned every chunk is
+// 16-byte aligned on both sides: the host decides that once (vec16) and the chunks are then copied with 128-bit accesses.
 //   mode 0 pack    : chunk (b, i, p): src ((b*n1loc + i)*n2 + p*n2blk)*n3        -> dst (((p*B + b)*n1loc + i)*n2blk)*n3,   clen = n2blk*n3
 //   mode 1 unpack  : chunk (p, b, i): src (((p*B + b)*n1blk + i)*n2loc)*n3       -> dst ((b*n1 + p*n1blk + i)*n2loc)*n3,    clen = n2loc*n3
 //   mode 2 pack_rev: chunk (b, p, i): src ((b*n1 + p*n1blk + i)*n2loc)*n3        -> dst (((p*B + b)*n1blk + i)*n2loc)*n3,   clen = n2loc*n3
 //   mode 3 unp_rev : chunk (p, b, i): src (((p*B + b)*n1loc + i)*n2blk)*n3       -> dst ((b*n1loc + i)*n2 + p*n2blk)*n3,    clen = n2blk*n3
-struct TrArgs { int64_t B, nA, nB, n3; int P; int mode; int64_t clen; };
+struct TrArgs { int64_t B, nA, nB, n3; int P; int mode; int64_t clen; int vec16; };
 
 __global__ void __launch_bounds__(256) k_tr_chunks(const double* __restrict__ src, double* __restrict__ dst, TrArgs a)
 {
@@ -511,7 +498,9 @@ __global__ void __launch_bounds__(256) k_tr_chunks(const double* __restrict__ sr
     const double* __restrict__ s = src + so;
     double* __restrict__ d = dst + dof;
     const int64_t start = (int64_t)blockIdx.y * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.y * blockDim.x;
-    if (((so | dof | a.clen) & 1) == 0) {
+    if (a.vec16) {
+        DB_CHECK_ALIGN16(s);
+        DB_CHECK_ALIGN16(d);
         const double2* __restrict__ s2 = reinterpret_cast<const double2*>(s);
         double2* __restrict__ d2 = reinterpret_cast<double2*>(d);
         for (int64_t e = start; e < (a.clen >> 1); e += stride) d2[e] = s2[e];
@@ -520,38 +509,40 @@ __global__ void __launch_bounds__(256) k_tr_chunks(const double* __restrict__ sr
     }
 }
 
+// modes 0 and 3 split nB (= n2) over the P peers, modes 1 and 2 nA (= n1)
 static int tr_launch(const double* src, double* dst, int mode, int64_t B, int64_t nA, int64_t nB, int64_t n3, int P, void* stream, const char* name)
 {
+    if (P < 1) { db_set_error("%s: P must be at least 1 (got %d)", name, P); return 1; }
+    const bool split_n2 = mode == 0 || mode == 3;
+    if ((split_n2 ? nB : nA) % P) { db_set_error("%s: %s not divisible by P", name, split_n2 ? "n2" : "n1"); return 1; }
     TrArgs a; a.B = B; a.nA = nA; a.nB = nB; a.n3 = n3; a.P = P; a.mode = mode;
     int64_t nchunks;
-    if (mode == 0 || mode == 3) { a.clen = (nB / P) * n3; nchunks = B * nA * P; }
+    if (split_n2) { a.clen = (nB / P) * n3; nchunks = B * nA * P; }
     else { a.clen = nB * n3; nchunks = B * nA; }
     if (nchunks <= 0 || a.clen <= 0) return 0;
     if (nchunks > 2147483647LL) { db_set_error("%s: too many chunks", name); return 1; }
+    a.vec16 = (a.clen % 2 == 0) && (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0);
     int64_t gy = (a.clen / 2 + 256 * 8 - 1) / (256 * 8);       // ~8 vector elements per thread
     if (gy < 1) gy = 1;
     if (gy > 64) gy = 64;
     DB_LAUNCH(k_tr_chunks, dim3((unsigned)nchunks, (unsigned)gy), dim3(256), 0, stream, src, dst, a);
+    ++g_pw_launches[a.vec16 ? 3 : 4];
     return db_check_launch(name);
 }
 
 extern "C" int db_transpose_pack(const double* a, double* sendbuf, int64_t B, int64_t n1loc, int64_t n2, int64_t n3, int32_t P, void* stream)
 {
-    if (n2 % P) { db_set_error("transpose_pack: n2 not divisible by P"); return 1; }
     return tr_launch(a, sendbuf, 0, B, n1loc, n2, n3, P, stream, "transpose_pack");
 }
 extern "C" int db_transpose_unpack(const double* recvbuf, double* out, int64_t B, int64_t n1, int64_t n2loc, int64_t n3, int32_t P, void* stream)
 {
-    if (n1 % P) { db_set_error("transpose_unpack: n1 not divisible by P"); return 1; }
     return tr_launch(recvbuf, out, 1, B, n1, n2loc, n3, P, stream, "transpose_unpack");
 }
 extern "C" int db_transpose_pack_rev(const double* a, double* sendbuf, int64_t B, int64_t n1, int64_t n2loc, int64_t n3, int32_t P, void* stream)
 {
-    if (n1 % P) { db_set_error("transpose_pack_rev: n1 not divisible by P"); return 1; }
     return tr_launch(a, sendbuf, 2, B, n1, n2loc, n3, P, stream, "transpose_pack_rev");
 }
 extern "C" int db_transpose_unpack_rev(const double* recvbuf, double* out, int64_t B, int64_t n1loc, int64_t n2, int64_t n3, int32_t P, void* stream)
 {
-    if (n2 % P) { db_set_error("transpose_unpack_rev: n2 not divisible by P"); return 1; }
     return tr_launch(recvbuf, out, 3, B, n1loc, n2, n3, P, stream, "transpose_unpack_rev");
 }

@@ -95,6 +95,7 @@ SIGNATURES = {
     "db_ragged_matvec": (C.c_int, [vp, vp, i32, i32, vp, vp, i64, i32, i32, i32, i32, i64, vp]),
     "db_pointwise": (C.c_int, [vp, vp, i64, i32, i32, vp, vp, vp, vp, i32, vp]),
     "db_pointwise_pairs": (C.c_int, [vp, vp, i64, i32, i32, vp, vp, vp]),
+    "db_pointwise_launches": (C.c_longlong, [i32]),
     "db_rfft_x_products": (C.c_int, [PFFT, vp, i64, vp, i64, i32, i64, f64, vp, i32, vp, i32, i32, vp]),
     "db_rfft_blocks_per_sm": (C.c_int, [i32, i32, i32, i32, i32]),
     "db_pencil_gather": (C.c_int, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp]),

@@ -146,13 +146,17 @@ int db_ragged_matvec(const double* mats, const db_ragged_entry* entries, int32_t
  * Replaces DotProduct.operate / MultiplyFields.operate / AddFields.operate chains
  * (core/arithmetic.py:246-251, 666-674, 855-866).
  * in: (n_in, npoints) stacked inputs, out: (n_out, npoints).  Program: for output o, terms
- * term_ptr[o]..term_ptr[o+1]; term t has coefficient coef[t] and factors fac[fac_ptr[t]..fac_ptr[t+1]). */
+ * term_ptr[o]..term_ptr[o+1]; term t has coefficient coef[t] and factors fac[fac_ptr[t]..fac_ptr[t+1]).
+ * At most 113 inputs (a tile of 256 points of every input in shared memory); more return 1 with a message.  An even npoints with
+ * 16-byte aligned in and out and at most 56 inputs takes the double-buffered two-points-per-thread kernel, everything else the
+ * single-buffered one; both evaluate the same arithmetic, so their results are bitwise equal.  npoints <= 0 or n_out <= 0: nothing. */
 int db_pointwise(const double* in, double* out, int64_t npoints, int32_t n_in, int32_t n_out,
                  const int32_t* term_ptr, const double* coef, const int32_t* fac_ptr, const int32_t* fac, int32_t nfac_total,
                  void* stream);
 /* The same for programs whose terms have one or two factors (quadratic nonlinearities): term t of output o
- * (term_ptr[o] <= t < term_ptr[o+1]) is coef * in[a] * in[b], or coef * in[a] when b < 0.  npoints even, arrays
- * 16-byte aligned. */
+ * (term_ptr[o] <= t < term_ptr[o+1]) is coef * in[a] * in[b], or coef * in[a] when b < 0, accumulated as fma(coef * in[a], in[b], acc).
+ * npoints even, at most 56 inputs, and in, out and terms 16-byte aligned (terms are read as 16-byte records); otherwise returns 1
+ * with a message. */
 typedef struct { double coef; int32_t a; int32_t b; } db_pair_term;
 int db_pointwise_pairs(const double* in, double* out, int64_t npoints, int32_t n_in, int32_t n_out,
                        const int32_t* term_ptr, const db_pair_term* terms, void* stream);
@@ -327,6 +331,14 @@ int db_transpose_pack(const double* a, double* sendbuf, int64_t B, int64_t n1loc
 int db_transpose_unpack(const double* recvbuf, double* out, int64_t B, int64_t n1, int64_t n2loc, int64_t n3, int32_t P, void* stream);
 int db_transpose_pack_rev(const double* a, double* sendbuf, int64_t B, int64_t n1, int64_t n2loc, int64_t n3, int32_t P, void* stream);
 int db_transpose_unpack_rev(const double* recvbuf, double* out, int64_t B, int64_t n1loc, int64_t n2, int64_t n3, int32_t P, void* stream);
+/* All four: P >= 1 and the split axis (n2 for pack / unpack_rev, n1 for unpack / pack_rev) divisible by P, else 1 with a message;
+ * B, n1 or n3 = 0: nothing.  A chunk (n2blk * n3 or n2loc * n3 doubles) is copied with 16-byte accesses when its length is even and
+ * both base pointers are 16-byte aligned, with 8-byte accesses otherwise. */
+
+/* diagnostic: launches so far of the kernels behind db_pointwise, db_pointwise_pairs and the transposes, by kind: 0 the
+ * single-buffered general kernel, 1 the double-buffered general kernel, 2 the pairs kernel, 3 a transpose with 16-byte accesses,
+ * 4 a transpose with 8-byte accesses; -1 for any other kind */
+long long db_pointwise_launches(int32_t kind);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Curvilinear pencil path (SURVEY section 8f rank 2: sphere / shell problems).  On the sphere the pencils are one system

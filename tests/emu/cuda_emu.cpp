@@ -199,6 +199,10 @@ void bulk_land(const BulkCopy& c) {
 }
 }  // namespace
 
+void emu_check_align16(const void* p, const char* what) {
+    if ((uintptr_t)p % 16) emu_fail("%s: 16-byte access at %p, which is not 16-byte aligned", what, p);
+}
+
 void emu_mbar_init(unsigned long long* bar) {
     check_bar(bar, "mbarrier.init");
     *bar = 0;

@@ -77,6 +77,10 @@ void emu_cp_async_zfill(void* dst, const void* src, size_t bytes, size_t src_byt
 void emu_cp_commit();                // close the open group (also when it is empty), as cp.async.commit_group
 void emu_cp_wait(int n);             // land every committed group except the n most recent, as cp.async.wait_group n
 
+// a 16-byte global load or store (double2) at p, in kernel `what`: aborts with a message unless p is 16-byte aligned (the GPU faults
+// with a misaligned address there, while host memory would take it silently)
+void emu_check_align16(const void* p, const char* what);
+
 // a statically sized __shared__ array (DB_SHARED_ARRAY): one host array shared by the fibers; the first thread of every block to reach
 // the declaration poisons it, as emu_launch poisons the dynamic shared memory
 void emu_static_smem(void* p, size_t bytes);

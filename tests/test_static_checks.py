@@ -39,12 +39,12 @@ def _constant(expr, defines):
         return None
 
 
-def test_every_launch_with_dynamic_shared_memory_above_48k_opts_in():
+def test_every_runtime_sized_launch_above_48k_opts_in():
     """A launch asking for more than 48 KB of dynamic shared memory fails on the GPU with 'invalid argument' unless the kernel was
     given cudaFuncAttributeMaxDynamicSharedMemorySize first; the emulation accepts anything up to the 227 KB hardware limit.  Every
     DB_LAUNCH whose size is not a compile-time constant <= 48 KB must have the attribute set for the same kernel in the same file."""
     common = (CSRC / "db_common.cuh").read_text()
-    checked = 0
+    checked = set()
     for f in sorted(CSRC.glob("*.cu")):
         text = f.read_text()
         defines = dict(re.findall(r"#define\s+([A-Z_0-9]+)\s+([0-9][0-9 *+()]*)\s*(?://.*)?$", common + "\n" + text, flags=re.M))
@@ -58,6 +58,8 @@ def test_every_launch_with_dynamic_shared_memory_above_48k_opts_in():
             val = _constant(smem_expr, defines)
             if val is not None and val <= 48 * 1024:
                 continue
-            checked += 1
+            checked.add(kern)
             assert kern in opted, f"{f.name}: {kern} is launched with dynamic shared memory '{smem_expr}' but never opts in above 48 KB"
-    assert checked >= 8, checked
+    # the launches with a run-time size (the parse must find every one of them)
+    assert checked >= {"k_banded_solve", "k_dense_solve", "k_band_lines", "k_batches_matvec", "k_pointwise", "k_pointwise_v3",
+                       "k_pointwise_pairs"}, checked
