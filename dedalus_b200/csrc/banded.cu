@@ -7,7 +7,6 @@
 // for a warp: pivot search = shuffle arg-max over the kl + 1 candidates, interchange and rank-1 update = lanes over the
 // (kl) x (ku + kl) window.  Vectors of system s: element (i, r) at vec_off + i * nrhs + r.
 #include "db_common.cuh"
-#include <cstdlib>
 
 #ifdef DB_EMU
 #define DB_WARP_SYNC() emu_yield()
@@ -26,25 +25,6 @@ __device__ __forceinline__ bool bd_finite(double v) { return v - v == 0.0; }
 #define BD_LDCG(p) __ldcg(p)
 #define BD_FENCE() __threadfence_block()
 #endif
-// Kernel variants (environment DB_BANDED_MODE or db_banded_set_mode; default 3):
-//   bit 0: the factor kernel re-reads band entries that other lanes wrote with L2 loads (ld.global.cg) behind a CTA fence
-//          instead of relying on the SM's L1 for lane-to-lane communication through global memory;
-//   bit 1: the solve kernel reads the factor columns straight from global memory instead of through the cp.async ring.
-// A backward error of 1.2e-5 seen once from variant 0 is explained by a race in the solve's cp.async ring: when its prologues
-// committed fewer than BS_DEPTH - 1 groups (n < BS_DEPTH - 1; n = 2 NC = 6 for the m = Lmax system of the stock shallow-water
-// problem), the wait of step j did not cover column j, so the forward sweep could read L columns that had not landed and the
-// backward sweep a ring slot still holding a forward-sweep column.  tests/test_emu_banded.py, where emulated copies land only
-// when their group is retired, checks every variant at those sizes.  Whether the ring solve is faster has not been measured, so
-// the variant without asynchronous copies stays the default, and dedalus_b200/sphere.py SphereSystems.factor_verified still
-// verifies (and retries) every factorisation.
-static int g_bd_mode = -1;
-static int bd_mode()
-{
-    if (g_bd_mode < 0) { const char* e = getenv("DB_BANDED_MODE"); g_bd_mode = e ? atoi(e) : 3; }
-    return g_bd_mode;
-}
-extern "C" int db_banded_set_mode(int32_t mode) { g_bd_mode = mode; return 0; }
-
 #define BD_WARPS 4            // systems per CTA in the factor / elementwise kernels
 
 // ---------------------------------------------------------------------------------------------------------
@@ -82,7 +62,7 @@ extern "C" int db_banded_combine(const db_banded_sys* sys, int32_t nsys, int32_t
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(32 * BD_WARPS)
 k_banded_factor(const db_banded_sys* __restrict__ sys, int nsys, int kl, int ku, double* ab_all,
-                int32_t* __restrict__ ipiv_all, int32_t* __restrict__ info, int cg)
+                int32_t* __restrict__ ipiv_all, int32_t* __restrict__ info)
 {
     const int lane = threadIdx.x & 31;
     const int s = blockIdx.x * BD_WARPS + (threadIdx.x >> 5);
@@ -94,15 +74,15 @@ k_banded_factor(const db_banded_sys* __restrict__ sys, int nsys, int kl, int ku,
     double* ab = ab_all + S.lu_off;
     int32_t* __restrict__ ipiv = ipiv_all + S.piv_off;
     int ju = 0, bad = 0;
-#define BD_RD(ptr) (cg ? BD_LDCG(ptr) : *(ptr))
-#define BD_SYNC() do { if (cg) BD_FENCE(); DB_WARP_SYNC(); } while (0)
+    // band entries that other lanes wrote are re-read from L2 (ld.global.cg) behind a CTA fence, not through the SM's L1
+#define BD_SYNC() do { BD_FENCE(); DB_WARP_SYNC(); } while (0)
     for (int j = 0; j < n; ++j) {
         const int km = bd_min(kl, n - 1 - j);
         double* colj = ab + (int64_t)j * ldf + kv;                       // colj[l] = A(j + l, j)
         // pivot search: largest |A(j + l, j)|, l = 0 .. km, lowest l on ties
         double best = -1.0; int bl = 0;
         for (int l = lane; l <= km; l += 32) {
-            const double v = fabs(BD_RD(colj + l));
+            const double v = fabs(BD_LDCG(colj + l));
             if (v > best) { best = v; bl = l; }
         }
 #pragma unroll
@@ -120,13 +100,13 @@ k_banded_factor(const db_banded_sys* __restrict__ sys, int nsys, int kl, int ku,
         if (jp != 0) {
             for (int c = j + lane; c <= ju; c += 32) {
                 double* p = ab + (int64_t)c * ldf + kv + (j - c);
-                const double t = BD_RD(p), u = BD_RD(p + jp); p[0] = u; p[jp] = t;
+                const double t = BD_LDCG(p), u = BD_LDCG(p + jp); p[0] = u; p[jp] = t;
             }
         }
         BD_SYNC();
-        const double rp = 1.0 / BD_RD(colj);
+        const double rp = 1.0 / BD_LDCG(colj);
         BD_SYNC();
-        for (int l = 1 + lane; l <= km; l += 32) colj[l] = BD_RD(colj + l) * rp;
+        for (int l = 1 + lane; l <= km; l += 32) colj[l] = BD_LDCG(colj + l) * rp;
         BD_SYNC();
         // trailing update A(j + l, c) -= L(l) * U(j, c),  l = 1 .. km,  c = j + 1 .. ju
         const int nc = ju - j;
@@ -134,11 +114,10 @@ k_banded_factor(const db_banded_sys* __restrict__ sys, int nsys, int kl, int ku,
             const int cc = idx / km, l = 1 + idx - cc * km;
             const int c = j + 1 + cc;
             double* p = ab + (int64_t)c * ldf + kv + (j - c);             // p[0] = U(j, c), p[l] = A(j + l, c)
-            p[l] = fma(-BD_RD(colj + l), BD_RD(p), BD_RD(p + l));
+            p[l] = fma(-BD_LDCG(colj + l), BD_LDCG(p), BD_LDCG(p + l));
         }
         BD_SYNC();
     }
-#undef BD_RD
 #undef BD_SYNC
     if (live && lane == 0) info[s] = bad;
 }
@@ -148,7 +127,7 @@ extern "C" int db_banded_factor(const db_banded_sys* sys, int32_t nsys, int32_t 
 {
     if (nsys <= 0) return 0;
     DB_LAUNCH(k_banded_factor, dim3((unsigned)((nsys + BD_WARPS - 1) / BD_WARPS)), dim3(32 * BD_WARPS), 0, stream,
-              sys, nsys, kl, ku, ab, ipiv, info, bd_mode() & 1);
+              sys, nsys, kl, ku, ab, ipiv, info);
     return db_check_launch("banded_factor");
 }
 
@@ -156,14 +135,12 @@ extern "C" int db_banded_factor(const db_banded_sys* sys, int32_t nsys, int32_t 
 // Solve  x = A^{-1} (sum_k coef_k v_k)  for every right-hand-side column, both triangular sweeps in one launch.
 // CTA = one warp = one (system, chunk of RC columns).  The right-hand side (combined on the fly from up to 16 vectors: the
 // IMEX stage combination of core/timesteppers.py:617-623) is staged ONCE in shared memory, both sweeps run there, and the
-// factor columns stream through a shared-memory ring filled DEPTH columns ahead by cp.async, so neither the vector nor the
-// factor loads sit on the dependent chain of the sweep.
+// factor columns are read straight from global memory.
 // ---------------------------------------------------------------------------------------------------------
-#define BS_DEPTH 8
 
 __global__ void __launch_bounds__(32)
 k_banded_solve(const db_banded_sys* __restrict__ sys, int kl, int ku, const double* __restrict__ ab_all,
-               const int32_t* __restrict__ ipiv_all, db_veccomb rhs, double* __restrict__ x_all, int RC, int direct)
+               const int32_t* __restrict__ ipiv_all, db_veccomb rhs, double* __restrict__ x_all, int RC)
 {
     DB_SMEM(double, smem);
     const db_banded_sys S = sys[blockIdx.x];
@@ -174,8 +151,7 @@ k_banded_solve(const db_banded_sys* __restrict__ sys, int kl, int ku, const doub
     const int R = bd_min(RC, nrhs - r0);
     const int kv = kl + ku, ldf = 2 * kl + ku + 1;
     double* __restrict__ b = smem;                                   // [n][R]
-    double* __restrict__ ring = smem + (int64_t)n * RC;              // [BS_DEPTH][ldf]
-    int32_t* __restrict__ piv = reinterpret_cast<int32_t*>(ring + BS_DEPTH * ldf);     // [n]
+    int32_t* __restrict__ piv = reinterpret_cast<int32_t*>(smem + (int64_t)n * RC);     // [n]
     const double* __restrict__ ab = ab_all + S.lu_off;
     // stage: combined right-hand side and the pivot rows
     for (int64_t e = lane; e < (int64_t)n * R; e += 32) {
@@ -187,30 +163,15 @@ k_banded_solve(const db_banded_sys* __restrict__ sys, int kl, int ku, const doub
     }
     for (int i = lane; i < n; i += 32) piv[i] = ipiv_all[S.piv_off + i] - i;
     // ---- forward sweep: y = L^{-1} P b
-    // Both prologues commit exactly BS_DEPTH - 1 groups, empty ones past the last column, so that group j always holds column j
-    // and the wait of step j (all but the BS_DEPTH - 1 newest groups) covers it for every n.
-    for (int d = 0; d < BS_DEPTH - 1 && !direct; ++d) {
-        if (d < n)
-            for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[d * ldf + l], &ab[(int64_t)d * ldf + l]);
-        db_cp_commit();
-    }
     DB_WARP_SYNC();
     for (int j = 0; j < n; ++j) {
-        const int jn = j + BS_DEPTH - 1;
-        if (!direct) {
-            if (jn < n)
-                for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[(jn % BS_DEPTH) * ldf + l], &ab[(int64_t)jn * ldf + l]);
-            db_cp_commit();
-            db_cp_wait<BS_DEPTH - 1>();
-        }
-        DB_WARP_SYNC();
         const int km = bd_min(kl, n - 1 - j);
         const int p = piv[j];
         if (p != 0) {
             for (int r = lane; r < R; r += 32) { const double t = b[j * R + r]; b[j * R + r] = b[(j + p) * R + r]; b[(j + p) * R + r] = t; }
             DB_WARP_SYNC();
         }
-        const double* col = direct ? ab + (int64_t)j * ldf + kv : ring + (j % BS_DEPTH) * ldf + kv;
+        const double* col = ab + (int64_t)j * ldf + kv;
         for (int idx = lane; idx < km * R; idx += 32) {
             const int l = 1 + idx / R, r = idx % R;
             b[(j + l) * R + r] = fma(-col[l], b[j * R + r], b[(j + l) * R + r]);
@@ -218,25 +179,8 @@ k_banded_solve(const db_banded_sys* __restrict__ sys, int kl, int ku, const doub
         DB_WARP_SYNC();
     }
     // ---- backward sweep: x = U^{-1} y  (column oriented: x_j = y_j / U_jj, then y_i -= U_ij x_j for i = j - kv .. j - 1)
-    db_cp_wait<0>();
-    DB_WARP_SYNC();
-    for (int d = 0; d < BS_DEPTH - 1 && !direct; ++d) {
-        if (d < n)
-            for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[d * ldf + l], &ab[(int64_t)(n - 1 - d) * ldf + l]);
-        db_cp_commit();
-    }
-    DB_WARP_SYNC();
-    for (int jj = 0; jj < n; ++jj) {
-        const int j = n - 1 - jj;
-        const int jn = jj + BS_DEPTH - 1;
-        if (!direct) {
-            if (jn < n)
-                for (int l = lane; l < ldf; l += 32) db_cp_async8(&ring[(jn % BS_DEPTH) * ldf + l], &ab[(int64_t)(n - 1 - jn) * ldf + l]);
-            db_cp_commit();
-            db_cp_wait<BS_DEPTH - 1>();
-        }
-        DB_WARP_SYNC();
-        const double* col = direct ? ab + (int64_t)j * ldf + kv : ring + (jj % BS_DEPTH) * ldf + kv;      // col[i - j] = U(i, j), i <= j
+    for (int j = n - 1; j >= 0; --j) {
+        const double* col = ab + (int64_t)j * ldf + kv;                  // col[i - j] = U(i, j), i <= j
         const double rd = 1.0 / col[0];
         for (int r = lane; r < R; r += 32) b[j * R + r] *= rd;
         DB_WARP_SYNC();
@@ -247,7 +191,6 @@ k_banded_solve(const db_banded_sys* __restrict__ sys, int kl, int ku, const doub
         }
         DB_WARP_SYNC();
     }
-    db_cp_wait<0>();
     for (int64_t e = lane; e < (int64_t)n * R; e += 32) {
         const int64_t i = e / R; const int r = (int)(e - i * R);
         x_all[S.vec_off + i * nrhs + r0 + r] = b[i * R + r];
@@ -259,16 +202,15 @@ extern "C" int db_banded_solve(const db_banded_sys* sys, int32_t nsys, int32_t k
 {
     if (nsys <= 0 || max_n <= 0 || max_nrhs <= 0) return 0;
     if (rhs->nvec < 1 || rhs->nvec > 16) { db_set_error("banded_solve: 1..16 right-hand-side vectors"); return 1; }
-    const int ldf = 2 * kl + ku + 1;
-    // columns per CTA: as many as fit 96 KB next to the factor ring (the sweeps of different chunks are independent)
+    // columns per CTA: as many as fit 96 KB (the sweeps of different chunks are independent)
     int RC = max_nrhs < 8 ? max_nrhs : 8;
     while (RC > 1 && (size_t)max_n * RC * 8 > 96 * 1024) RC >>= 1;
-    const size_t smem = ((size_t)max_n * RC + (size_t)BS_DEPTH * ldf) * sizeof(double) + (size_t)max_n * sizeof(int32_t);
+    const size_t smem = (size_t)max_n * RC * sizeof(double) + (size_t)max_n * sizeof(int32_t);
     if (smem > DB_MAX_SMEM) { db_set_error("banded_solve: system of size %d does not fit shared memory", max_n); return 1; }
     static bool attr_set = false;
     if (!attr_set) { DB_SET_SMEM_ATTR(k_banded_solve); attr_set = true; }
     DB_LAUNCH(k_banded_solve, dim3((unsigned)nsys, (unsigned)((max_nrhs + RC - 1) / RC)), dim3(32), smem, stream,
-              sys, kl, ku, ab, ipiv, *rhs, x, RC, (bd_mode() >> 1) & 1);
+              sys, kl, ku, ab, ipiv, *rhs, x, RC);
     return db_check_launch("banded_solve");
 }
 

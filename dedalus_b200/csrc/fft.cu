@@ -715,7 +715,6 @@ static int launch_fft(const db_fft_plan* plan, const double* in, double* out, in
     // choose the tile width: up to 16 lines, shrunk until the CTA fits ~110 KB (2 CTAs / SM) or, failing that,
     // the 227 KB per-CTA limit
     int T = 16;
-    { const char* e = getenv("DB_FFT_T"); if (e) { int v = atoi(e); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16 || v == 32) T = v; } }
     const int64_t lines_dir = (inner == 1) ? outer : inner;
     // work-buffer rows (doubles per column): the complex FFT buffer, which the Chebyshev backward kernel also uses
     // as scratch for n_coeff staged coefficients

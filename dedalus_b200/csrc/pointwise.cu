@@ -374,10 +374,8 @@ extern "C" int db_mmt_apply(const double* mat, int32_t m, int32_t n, const doubl
 {
     if (outer <= 0 || inner <= 0 || m <= 0 || n <= 0) return 0;
     if (outer > 65535) { db_set_error("mmt_apply: outer too large (%lld)", (long long)outer); return 1; }
-    static int dmma = -1;
-    if (dmma < 0) { const char* e = getenv("DB_MMT_DMMA"); dmma = (e && atoi(e) == 0) ? 0 : 1; }
     const bool aligned = (((uintptr_t)mat | (uintptr_t)in | (uintptr_t)out) & 15) == 0;
-    if (dmma && aligned && n % 2 == 0 && inner % 2 == 0) {
+    if (aligned && n % 2 == 0 && inner % 2 == 0) {
         dim3 grid((unsigned)((inner + DM_BN - 1) / DM_BN), (unsigned)((m + DM_BM - 1) / DM_BM), (unsigned)outer);
         DB_LAUNCH(k_mmt_dmma, grid, dim3(128), 0, stream, mat, m, n, in, out, inner);
         ++g_mmt_dmma_launches;

@@ -14,7 +14,6 @@
 // Conventions as in fft.cu (reference core/transforms.py:469-509, 537-565): cos / -sin interleaved coefficients,
 // forward scaled by 2/n (1/n for k = 0), sin(0) slot zero, Nyquist dropped.
 #include "db_common.cuh"
-#include <cstdlib>
 #include <utility>
 #include "tw96.inc"
 
@@ -140,10 +139,11 @@ __device__ __forceinline__ double2 ldtwn(const double* __restrict__ tw, int j) {
 __device__ __forceinline__ double2 cmulc2(double2 a, double2 w) { return make_double2(a.x * w.x + a.y * w.y, a.y * w.x - a.x * w.y); }
 __device__ __forceinline__ double2 cmul2(double2 a, double2 w) { return make_double2(a.x * w.x - a.y * w.y, a.x * w.y + a.y * w.x); }
 
-// Tile height: P complex line pairs (2P real lines) per CTA tile, P = 8 or 4.  The per-pair arithmetic does not depend on P,
-// so both tile heights give bitwise-equal results; smaller tiles mean smaller CTAs, more of them per SM in different phases.
-// Both divide the 16 lines the coverage tests below require of `inner`.
-#define RR_LINES 16
+// Tile height: P complex line pairs (2P real lines) per CTA tile.  The kernels take P as a template parameter; the Fourier
+// launches below build them at RR_P = 8 only (half-height tiles were measured slower, DESIGN section 4).  The tile's 16 lines are
+// what the coverage tests below require of `inner`.
+#define RR_P 8
+#define RR_LINES (2 * RR_P)
 
 // Persistent CTAs walk the tiles (tile = 2P adjacent lines x the whole line length) with the NEXT tile's input rows in
 // flight (16-byte cp.async, L1-bypassing) while the current tile is transformed: two shared-memory buffers of
@@ -169,7 +169,7 @@ __device__ __forceinline__ void stage_rows(double* buf, const double* __restrict
 //   stage B (size NB):      thread (h, k1, p) computes the NB/2 outputs k2 = 2 m + h (first radix-2 split, DIF)
 // (forward: the same two splits in the opposite order).  3 NB P threads work in stage A and 6 Q P in stage B: 384 = 384
 // at n = 384 and P = 8, at ~80 registers, so two CTAs (24 warps) are resident per SM and every warp works in both stages.
-// minb() keeps 768 threads per SM at every P (the same register budget per thread) where shared memory allows.  The forward and
+// minb() keeps 768 threads per SM (the same register budget per thread at any P) where shared memory allows.  The forward and
 // the derivative backward transforms of lines of 192 or more points need more than the ~80 registers that leaves: they spill
 // (320 and 460 bytes at n = 384) and run at about half the bandwidth of the plain backward.  minb(true) gives them the whole
 // register file of one CTA (no spills in the forward, 88 bytes in the backward), which is faster despite the single CTA per SM;
@@ -661,13 +661,15 @@ struct ChebArgs {
 };
 
 // Tile height.  The z kernels are one tile per CTA with full-CTA barriers between their phases, i.e. latency-bound at
-// 2 CTAs / SM (long-scoreboard stalls): P = line pairs per tile is a template parameter so that
-// smaller tiles (P = 4: 8 lines, 192 threads, 49 KB at n = 384 -> 4 CTAs / SM in different phases) can hide it.
+// 2 CTAs / SM (long-scoreboard stalls): P = line pairs per tile is a template parameter so that lines of 192 points or more
+// take smaller tiles (P = 4: 8 lines, 192 threads, 49 KB at n = 384 -> 4 CTAs / SM in different phases) that hide it;
+// shorter lines keep P = 8 (launch_cheb).
 template <int Q, int NB, int P> struct ChGeom {
+    static_assert(P == 8 || P == 4, "Chebyshev tiles are 8 or 4 line pairs high");
     static constexpr int NA = 3 * Q, N = NA * NB, LINES = 2 * P;
     static constexpr int TA = 3 * NB * P, TB = 6 * Q * P;
     static constexpr int THREADS = TA > TB ? TA : TB;
-    static constexpr int LOGP = P == 8 ? 3 : P == 4 ? 2 : P == 2 ? 1 : 0;
+    static constexpr int LOGP = P == 8 ? 3 : 2;
     static constexpr size_t SMEM = (size_t)LINES * (N + 2) * sizeof(double) + (size_t)N * P * sizeof(double2);
     static constexpr int MINB = (int)((226 * 1024) / (SMEM + 1024)) > 8 ? 8 : ((int)((226 * 1024) / (SMEM + 1024)) < 1 ? 1 : (int)((226 * 1024) / (SMEM + 1024)));
 };
@@ -976,9 +978,11 @@ k_chfwd_regs(ChebArgs a)
     }
 }
 
-template <int Q, int NB, int P>
-int launch_cheb_p(bool fwd, const ChebArgs& a, void* stream)
+template <int Q, int NB>
+int launch_cheb(bool fwd, const ChebArgs& a, void* stream)
 {
+    // small transforms keep the tall tile (their CTAs are small anyway)
+    constexpr int P = 3 * Q * NB < 192 ? 8 : 4;
     using G = ChGeom<Q, NB, P>;
     const int64_t blocks = (a.lines + G::LINES - 1) / G::LINES;
 #ifndef DB_EMU
@@ -996,25 +1000,6 @@ int launch_cheb_p(bool fwd, const ChebArgs& a, void* stream)
     return db_check_launch(fwd ? "cheb_forward(regs)" : "cheb_backward(regs)");
 }
 
-static int cheb_tile_pairs()
-{
-    static int p = 0;
-    if (p == 0) { const char* e = getenv("DB_CHEB_P"); p = e ? atoi(e) : 4; if (p != 8 && p != 4 && p != 2) p = 4; }
-    return p;
-}
-
-template <int Q, int NB>
-int launch_cheb(bool fwd, const ChebArgs& a, void* stream)
-{
-    // small transforms keep the tall tile (their CTAs are small anyway); the tile height of the long ones is tunable
-    if (3 * Q * NB < 192) return launch_cheb_p<Q, NB, 8>(fwd, a, stream);
-    switch (cheb_tile_pairs()) {
-        case 8: return launch_cheb_p<Q, NB, 8>(fwd, a, stream);
-        case 2: return launch_cheb_p<Q, NB, 2>(fwd, a, stream);
-        default: return launch_cheb_p<Q, NB, 4>(fwd, a, stream);
-    }
-}
-
 static int regs_num_sms()
 {
 #ifdef DB_EMU
@@ -1022,15 +1007,6 @@ static int regs_num_sms()
 #else
     return db_num_sms();
 #endif
-}
-
-// Tile heights (line pairs per tile) at n = 192 and 384 of the standalone transforms (DB_FFT_P = 8 | 4) and of the fused x pass
-// (DB_XPROD_P = 8 | 4); shorter lines always take P = 8.  P = 8 is the faster of the two for both (DESIGN section 4).  Read at
-// every launch, so that one process can time the variants against each other.
-static int tile_pairs(const char* env, int n)
-{
-    const char* e = n >= 192 && n <= 384 ? getenv(env) : nullptr;
-    return e && atoi(e) == 4 ? 4 : 8;
 }
 
 // CTAs of `kern` resident on one SM: the persistent grids launch exactly this many per SM (more would run as a second wave)
@@ -1046,12 +1022,13 @@ template <class K> int resident_per_sm(K kern, int threads, size_t bytes, int fi
 #endif
 }
 
-template <int Q, int NB, int P>
-size_t regs_smem() { return (size_t)2 * 3 * Q * NB * P * sizeof(double2); }
+template <int Q, int NB>
+size_t regs_smem() { return (size_t)2 * 3 * Q * NB * RR_P * sizeof(double2); }
 
-template <int Q, int NB, int P>
+template <int Q, int NB>
 void regs_attrs()
 {
+    constexpr int P = RR_P;
 #ifndef DB_EMU
     static bool attr = false;
     if (!attr) {
@@ -1066,11 +1043,11 @@ void regs_attrs()
 #endif
 }
 
-template <int Q, int NB, int P>
-int launch_regs_p(bool fwd, const RegArgs& a, int64_t outer, void* stream)
+template <int Q, int NB>
+int launch_regs(bool fwd, const RegArgs& a, int64_t outer, void* stream)
 {
-    constexpr int THREADS = RegGeom<Q, NB, P>::THREADS;
-    const size_t bytes = regs_smem<Q, NB, P>();
+    constexpr int P = RR_P, THREADS = RegGeom<Q, NB, P>::THREADS;
+    const size_t bytes = regs_smem<Q, NB>();
     TileWalk w;
     w.tiles_per_outer = a.inner / (2 * P);
     w.total = w.tiles_per_outer * outer;
@@ -1079,7 +1056,7 @@ int launch_regs_p(bool fwd, const RegArgs& a, int64_t outer, void* stream)
     int per_sm = (int)((size_t)(226 * 1024) / (bytes + 1024));
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 8) per_sm = 8;
-    regs_attrs<Q, NB, P>();
+    regs_attrs<Q, NB>();
     if (fwd) per_sm = resident_per_sm(k_rfwd_regs<Q, NB, P>, THREADS, bytes, per_sm);
     else if (a.deriv > 0) per_sm = resident_per_sm(k_rbwd_regs<Q, NB, P, true>, THREADS, bytes, per_sm);
     else per_sm = resident_per_sm(k_rbwd_regs<Q, NB, P, false>, THREADS, bytes, per_sm);
@@ -1092,19 +1069,11 @@ int launch_regs_p(bool fwd, const RegArgs& a, int64_t outer, void* stream)
     return db_check_launch(fwd ? "rfft_forward(regs)" : "rfft_backward(regs)");
 }
 
-template <int Q, int NB>
-int launch_regs(bool fwd, const RegArgs& a, int64_t outer, void* stream)
-{
-    if constexpr (3 * Q * NB >= 192 && 3 * Q * NB <= 384) {
-        if (tile_pairs("DB_FFT_P", 3 * Q * NB) == 4) return launch_regs_p<Q, NB, 4>(fwd, a, outer, stream);
-    }
-    return launch_regs_p<Q, NB, 8>(fwd, a, outer, stream);
-}
-
 // CTAs per SM of the fused x pass (its persistent grid is this times the SM count)
-template <int Q, int NB, int P>
+template <int Q, int NB>
 int x_products_per_sm(size_t bytes)
 {
+    constexpr int P = RR_P;
     using X = XpGeom<Q, NB, P>;
     int fit = (int)((size_t)(226 * 1024) / (bytes + 1024));
     if (fit > X::MINB) fit = X::MINB;
@@ -1120,9 +1089,10 @@ int x_products_per_sm(size_t bytes)
     return resident_per_sm(k_rfft_x_products<Q, NB, P>, X::THREADS, bytes, fit);
 }
 
-template <int Q, int NB, int P>
-int launch_x_products_p(const XProdArgs& a, int32_t n_held, void* stream)
+template <int Q, int NB>
+int launch_x_products(const XProdArgs& a, int32_t n_held, void* stream)
 {
+    constexpr int P = RR_P;
     using X = XpGeom<Q, NB, P>;
     const size_t bytes = X::smem(a.M, n_held);
     if (bytes > (size_t)DB_MAX_SMEM) {
@@ -1130,42 +1100,24 @@ int launch_x_products_p(const XProdArgs& a, int32_t n_held, void* stream)
         return 1;
     }
     const int64_t total = a.inner / (2 * P);
-    int64_t nblk = (int64_t)regs_num_sms() * x_products_per_sm<Q, NB, P>(bytes);
+    int64_t nblk = (int64_t)regs_num_sms() * x_products_per_sm<Q, NB>(bytes);
     if (nblk > total) nblk = total;
     DB_LAUNCH((k_rfft_x_products<Q, NB, P>), dim3((unsigned)nblk), dim3(X::THREADS), bytes, stream, a, total);
     return db_check_launch("rfft_x_products");
 }
 
 template <int Q, int NB>
-int launch_x_products(const XProdArgs& a, int32_t n_held, void* stream)
+int blocks_per_sm(int kind, int32_t n_coeff, int32_t n_held)
 {
-    if constexpr (3 * Q * NB >= 192 && 3 * Q * NB <= 384) {
-        if (tile_pairs("DB_XPROD_P", 3 * Q * NB) == 4) return launch_x_products_p<Q, NB, 4>(a, n_held, stream);
-    }
-    return launch_x_products_p<Q, NB, 8>(a, n_held, stream);
-}
-
-template <int Q, int NB, int P>
-int blocks_per_sm_p(int kind, int32_t n_coeff, int32_t n_held)
-{
-    if (kind == 2) return x_products_per_sm<Q, NB, P>(XpGeom<Q, NB, P>::smem(n_coeff, n_held));
-    regs_attrs<Q, NB, P>();
-    const size_t bytes = regs_smem<Q, NB, P>();
+    constexpr int P = RR_P;
+    if (kind < 0 || kind > 2) return -1;
+    if (kind == 2) return x_products_per_sm<Q, NB>(XpGeom<Q, NB, P>::smem(n_coeff, n_held));
+    regs_attrs<Q, NB>();
+    const size_t bytes = regs_smem<Q, NB>();
     int fit = (int)((size_t)(226 * 1024) / (bytes + 1024));
     fit = fit < 1 ? 1 : (fit > 8 ? 8 : fit);
     if (kind == 1) return resident_per_sm(k_rfwd_regs<Q, NB, P>, RegGeom<Q, NB, P>::THREADS, bytes, fit);
     return resident_per_sm(k_rbwd_regs<Q, NB, P, false>, RegGeom<Q, NB, P>::THREADS, bytes, fit);
-}
-
-template <int Q, int NB>
-int blocks_per_sm(int kind, int32_t n_coeff, int32_t n_held, int P)
-{
-    if (kind < 0 || kind > 2) return -1;
-    if (P == 8) return blocks_per_sm_p<Q, NB, 8>(kind, n_coeff, n_held);
-    if constexpr (3 * Q * NB >= 192 && 3 * Q * NB <= 384) {
-        if (P == 4) return blocks_per_sm_p<Q, NB, 4>(kind, n_coeff, n_held);
-    }
-    return -1;
 }
 
 static long long g_regs_launches = 0;
@@ -1180,9 +1132,6 @@ int db_rfft_regs_try(bool fwd, const db_fft_plan* plan, const double* in, double
                      int32_t in_rpb, int64_t in_blk_stride, int32_t out_rpb, int64_t out_blk_stride,
                      int32_t out_peers, double* const* out_blk_ptr)
 {
-    static int enabled = -1;
-    if (enabled < 0) { const char* e = getenv("DB_FFT_REGS"); enabled = (e && atoi(e) == 0) ? 0 : 1; }
-    if (!enabled) return -1;
     const int n = plan->n;
     if (!plan->half || plan->twn == nullptr) return -1;
     if (inner < RR_LINES || inner % RR_LINES != 0 || deriv > 4) return -1;
@@ -1221,9 +1170,6 @@ int db_rfft_regs_try(bool fwd, const db_fft_plan* plan, const double* in, double
 int db_cheb_regs_try(bool fwd, const db_fft_plan* plan, const double* in, double* out, int64_t lines, int32_t n_coeff,
                      const double* diags, int32_t nd, const double* pre, int32_t npre, const double* sol2, void* stream)
 {
-    static int enabled = -1;
-    if (enabled < 0) { const char* e = getenv("DB_CHEB_REGS"); enabled = (e && atoi(e) == 0) ? 0 : 1; }
-    if (!enabled) return -1;
     const int n = plan->n;
     if (plan->twn == nullptr || plan->twq == nullptr) return -1;
     if (n_coeff % 2 != 0 || n_coeff < 2 || n_coeff > n || lines > 2147483647LL * 4) return -1;
@@ -1277,15 +1223,15 @@ extern "C" int db_rfft_x_products(const db_fft_plan* plan, const double* in, int
 }
 
 // Resident CTAs per SM of a register transform (kind 0: backward, 1: forward) or of the fused x pass (kind 2, with n_coeff rows
-// and n_held held factors) at n grid points and `tile_pairs` line pairs per tile; -1 where no such kernel exists.
-extern "C" int db_rfft_blocks_per_sm(int32_t kind, int32_t n, int32_t n_coeff, int32_t n_held, int32_t tile_pairs)
+// and n_held held factors) at n grid points; -1 where no such kernel exists.
+extern "C" int db_rfft_blocks_per_sm(int32_t kind, int32_t n, int32_t n_coeff, int32_t n_held)
 {
     switch (n) {
-        case 384: return blocks_per_sm<8, 16>(kind, n_coeff, n_held, tile_pairs);
-        case 192: return blocks_per_sm<4, 16>(kind, n_coeff, n_held, tile_pairs);
-        case 96:  return blocks_per_sm<4, 8>(kind, n_coeff, n_held, tile_pairs);
-        case 48:  return blocks_per_sm<2, 8>(kind, n_coeff, n_held, tile_pairs);
-        case 24:  return blocks_per_sm<2, 4>(kind, n_coeff, n_held, tile_pairs);
+        case 384: return blocks_per_sm<8, 16>(kind, n_coeff, n_held);
+        case 192: return blocks_per_sm<4, 16>(kind, n_coeff, n_held);
+        case 96:  return blocks_per_sm<4, 8>(kind, n_coeff, n_held);
+        case 48:  return blocks_per_sm<2, 8>(kind, n_coeff, n_held);
+        case 24:  return blocks_per_sm<2, 4>(kind, n_coeff, n_held);
         default: return -1;
     }
 }

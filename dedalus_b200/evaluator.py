@@ -308,7 +308,7 @@ class RHSPlan:
         from collections import Counter
         from .transforms import cached_plan, RealFourierTransform
         dim = self.dist.dim
-        if os.environ.get("DB_RHS_FUSED", "1") == "0" or os.environ.get("DB_FFT_REGS", "1") == "0":
+        if os.environ.get("DB_RHS_FUSED", "1") == "0":
             return None
         if self.P != 1 or dim < 2 or self.grid_leaves or self.broadcast_leaves or self.pairs is None:
             return None

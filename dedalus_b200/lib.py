@@ -97,7 +97,7 @@ SIGNATURES = {
     "db_pointwise_pairs": (C.c_int, [vp, vp, i64, i32, i32, vp, vp, vp]),
     "db_pointwise_launches": (C.c_longlong, [i32]),
     "db_rfft_x_products": (C.c_int, [PFFT, vp, i64, vp, i64, i32, i64, f64, vp, i32, vp, i32, i32, vp]),
-    "db_rfft_blocks_per_sm": (C.c_int, [i32, i32, i32, i32, i32]),
+    "db_rfft_blocks_per_sm": (C.c_int, [i32, i32, i32, i32]),
     "db_pencil_gather": (C.c_int, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp]),
     "db_pencil_scatter": (C.c_int, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp]),
     "db_pencil_matvec": (C.c_int, [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
@@ -120,7 +120,6 @@ SIGNATURES = {
     "db_banded_factor": (C.c_int, [vp, i32, i32, i32, vp, vp, vp, vp]),
     "db_banded_solve": (C.c_int, [vp, i32, i32, i32, i32, i32, vp, vp, C.POINTER(VecComb), vp, vp]),
     "db_banded_matvec": (C.c_int, [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
-    "db_banded_set_mode": (C.c_int, [i32]),
     "db_dense_combine": (C.c_int, [i32, i32, f64, vp, f64, vp, vp, vp]),
     "db_dense_factor": (C.c_int, [i32, i32, vp, vp, vp, vp]),
     "db_dense_solve": (C.c_int, [vp, i32, i32, i32, vp, vp, C.POINTER(VecComb), vp, vp]),

@@ -104,8 +104,7 @@ class RealFourierTransform:
     def blocked_supported(self, inner):
         """Mirror of the coverage test in csrc/rfft_regs.cu db_rfft_regs_try."""
         return (self.N in (24, 48, 96, 192, 384, 768) and self.M % 2 == 0 and self.M >= 2 and 3 * self.M <= 2 * self.N
-                and inner >= 16 and inner % 16 == 0 and os.environ.get("DB_FFT_REGS", "1") != "0"
-                and os.environ.get("DB_BLOCKED_TRANSPOSE", "1") != "0")
+                and inner >= 16 and inner % 16 == 0 and os.environ.get("DB_BLOCKED_TRANSPOSE", "1") != "0")
 
     def backward_blocked(self, c_ptr, g_ptr, outer, inner, device, deriv=0, in_block=(0, 0), out_block=(0, 0)):
         plan = DevicePlan(self.N, 'real', device)
@@ -134,10 +133,6 @@ class RealFourierTransform:
     # ---- the x pass of a quadratic right-hand side fused with its products (include/dedalus_b200.h db_rfft_x_products)
     _XP_GEOM = {24: (2, 4), 48: (2, 8), 96: (4, 8), 192: (4, 16), 384: (8, 16)}       # n -> (Q, NB) of csrc/rfft_regs.cu
 
-    def x_products_tile_pairs(self):
-        """Line pairs per tile of the fused x pass (csrc/rfft_regs.cu tile_pairs): 8, or 4 with DB_XPROD_P=4 at n = 192 and 384."""
-        return 4 if self.N in (192, 384) and os.environ.get("DB_XPROD_P", "8").strip() == "4" else 8
-
     def x_products_supported(self, inner, n_held):
         """Mirror of the coverage test of db_rfft_x_products and its shared-memory budget (XpGeom::smem)."""
         if self.N not in self._XP_GEOM or not (self.M % 2 == 0 and self.M >= 2 and 3 * self.M <= 2 * self.N):
@@ -145,7 +140,7 @@ class RealFourierTransform:
         if inner < 16 or inner % 16 != 0 or not 0 <= n_held <= 3:
             return False
         q, nb = self._XP_GEOM[self.N]
-        p = self.x_products_tile_pairs()
+        p = 8                                                       # line pairs per tile (RR_P)
         threads = max(3 * nb * p, 6 * q * p)
         smem = 16 * (self.N * p + self.M * p + n_held * (nb // 2) * threads)
         return smem <= 227 * 1024

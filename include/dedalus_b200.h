@@ -119,7 +119,7 @@ int db_band_lines(const double* in, double* out, int64_t lines, int32_t n,
  * Replaces SeparableMatrixTransform -> apply_dense (core/transforms.py:54-75, tools/array.py:104-129). */
 int db_mmt_apply(const double* mat, int32_t m, int32_t n, const double* in, double* out, int64_t outer, int64_t inner, void* stream);
 /* diagnostic: number of db_mmt_apply calls served by the FP64 tensor-core kernel so far (n and inner even, mat / in / out 16-byte
- * aligned, DB_MMT_DMMA not 0); every other call runs the FMA-pipe kernel */
+ * aligned); every other call runs the FMA-pipe kernel */
 long long db_mmt_dmma_launches(void);
 
 /* Ragged batch of dense matrix-vector products: the spin-weighted spherical harmonic colatitude transform.
@@ -175,9 +175,9 @@ int db_rfft_x_products(const db_fft_plan* plan, const double* in, int64_t in_str
                        int32_t n_coeff, int64_t inner, double kscale, const db_xprod_item* items, int32_t n_items,
                        const int32_t* loads, int32_t n_loads, int32_t n_held, void* stream);
 /* CTAs resident per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor on the current device) of the register real-Fourier
- * transforms at n grid points with tile_pairs line pairs per tile: kind 0 backward, 1 forward, 2 the fused x pass with n_coeff
- * rows and n_held held factors (its persistent grid is this many CTAs per SM).  -1 where there is no such kernel. */
-int db_rfft_blocks_per_sm(int32_t kind, int32_t n, int32_t n_coeff, int32_t n_held, int32_t tile_pairs);
+ * transforms at n grid points: kind 0 backward, 1 forward, 2 the fused x pass with n_coeff rows and n_held held factors (its
+ * persistent grid is this many CTAs per SM).  -1 where there is no such kernel. */
+int db_rfft_blocks_per_sm(int32_t kind, int32_t n, int32_t n_coeff, int32_t n_held);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Pencil systems (S1-S4).  A batch holds S structurally identical systems of size n; one thread owns one system.
@@ -371,10 +371,6 @@ int db_banded_solve(const db_banded_sys* sys, int32_t nsys, int32_t kl, int32_t 
 /* ya = A x and / or yb = B x (operator storage; either output may be NULL): M.X, L.X of core/timesteppers.py:590-591 */
 int db_banded_matvec(const db_banded_sys* sys, int32_t nsys, int32_t kl, int32_t ku, const double* a_ab, const double* b_ab,
                      const double* x, double* ya, double* yb, void* stream);
-/* diagnostic variants of the two kernels above (also environment DB_BANDED_MODE): bit 0 = the factorisation re-reads entries
- * written by other lanes through L2 behind a CTA fence, bit 1 = the solve reads factor columns directly from global memory;
- * a negative mode returns to DB_BANDED_MODE (default 3) */
-int db_banded_set_mode(int32_t mode);
 /* gather (vec[e] = idx[e] >= 0 ? arena[idx[e]] : 0) / scatter (arena[idx[e]] = vec[e] where idx[e] >= 0) through an index
  * table: pencil vectors <-> coefficient arrays in the folded triangular (m, l) packing (core/subsystems.py:340-371) */
 int db_index_move(const int64_t* idx, int64_t count, double* arena, double* vec, int32_t gather, void* stream);

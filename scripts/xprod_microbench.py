@@ -1,13 +1,13 @@
-"""Time the fused x pass of the right-hand side (db_rfft_x_products) alone at the RB3D 256^3 shape, at every tile height, and the
-y-pass-shaped register transforms at both tile heights of the standalone kernels.
+"""Time the fused x pass of the right-hand side (db_rfft_x_products) alone at the RB3D 256^3 shape, and the y-pass-shaped register
+transforms.
 
 The fused pass runs the schedule of a real RB3D RHSPlan (15 inputs, 4 outputs, 3 held factors) on M = 256 coefficient rows of
-n = 384 points and inner = 384^2 random lines.  Each arm is timed with CUDA events over 20 launches after a warm-up; the arms are
-alternated in one process, 3 rounds, and the median round is reported.  Algorithmic traffic is every input and output array read
+n = 384 points and inner = 384^2 random lines.  Each kernel is timed with CUDA events over 20 launches after a warm-up, 3 rounds,
+and the median round is reported.  Algorithmic traffic is every input and output array read
 or written once.  Blocks per SM come from cudaOccupancyMaxActiveBlocksPerMultiprocessor (db_rfft_blocks_per_sm).
 
 usage: python scripts/xprod_microbench.py [--json PATH]"""
-import argparse, json, os, pathlib, statistics, subprocess, sys
+import argparse, json, pathlib, statistics, subprocess, sys
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parents[1]))
 import torch
 
@@ -33,18 +33,17 @@ def timed(fn):
     return e0.elapsed_time(e1) / LAUNCHES
 
 
-def run_arms(arms, make_fn):
-    """arms: {name: env}; make_fn() -> the launch closure.  Returns {name: [ms per round]}."""
-    fn = make_fn()
-    res = {name: [] for name in arms}
-    for name, env in arms.items():                     # warm-up: module load, attributes, first launch of every variant
-        os.environ.update(env); fn()
+def rounds(fn):
+    """ms per launch in each of ROUNDS rounds, after a warm-up launch (module load, attributes)."""
+    fn()
     torch.cuda.synchronize()
-    for _ in range(ROUNDS):
-        for name, env in arms.items():
-            os.environ.update(env)
-            res[name].append(timed(fn))
-    return res
+    return [timed(fn) for _ in range(ROUNDS)]
+
+
+def row(name, res, gb, bps):
+    ms = statistics.median(res)
+    print(f"{name:18s} {ms:12.3f} {min(res):8.3f} {max(res):8.3f} {gb / (ms * 1e-3):8.1f} {bps:8d}")
+    return dict(ms=res, gbps=gb / (ms * 1e-3), blocks_per_sm=bps)
 
 
 def main():
@@ -57,7 +56,7 @@ def main():
     from dedalus_b200.transforms import RealFourierTransform
     torch.cuda.set_device(0)
     lib = get_lib()
-    out = dict(card=card(), fused={}, y_pass={})
+    out = dict(card=card(), y_pass={})
     print(f"card: {out['card']}")
 
     # the RB3D schedule at a 384-point x line (the y and z sizes do not enter it)
@@ -73,19 +72,12 @@ def main():
     cin = torch.randn((n_src, M, inner), dtype=torch.float64, device='cuda')
     cout = torch.empty((n_out, M, inner), dtype=torch.float64, device='cuda')
     gb = 8 * (int(loads.numel()) + n_out) * M * inner / 1e9
-    arms = {f"P={p}": dict(DB_XPROD_P=str(p)) for p in (8, 4)}
-    res = run_arms(arms, lambda: (lambda: px.x_products(cin, cout, inner, xp['items'], xp['n_items'], loads, xp['n_held'])))
+    res = rounds(lambda: px.x_products(cin, cout, inner, xp['items'], xp['n_items'], loads, xp['n_held']))
     print(f"\nfused x pass: n = {n}, M = {M}, inner = {inner}, {loads.numel()} inputs, {n_out} outputs, {xp['n_held']} held, "
           f"{gb:.2f} GB per launch")
-    print(f"{'arm':18s} {'ms (median)':>12s} {'min':>8s} {'max':>8s} {'GB/s':>8s} {'CTAs/SM':>8s}")
-    for name, env in arms.items():
-        os.environ.update(env)
-        ms = statistics.median(res[name])
-        bps = lib._raw_db_rfft_blocks_per_sm(2, n, M, xp['n_held'], int(env['DB_XPROD_P']))
-        out['fused'][name] = dict(ms=res[name], gbps=gb / (ms * 1e-3), blocks_per_sm=bps)
-        print(f"{name:18s} {ms:12.3f} {min(res[name]):8.3f} {max(res[name]):8.3f} {gb / (ms * 1e-3):8.1f} {bps:8d}")
+    print(f"{'kernel':18s} {'ms (median)':>12s} {'min':>8s} {'max':>8s} {'GB/s':>8s} {'CTAs/SM':>8s}")
+    out['fused'] = row("fused", res, gb, lib._raw_db_rfft_blocks_per_sm(2, n, M, xp['n_held']))
     del cin, cout
-    os.environ.pop("DB_XPROD_P")
 
     # y pass of RB3D 256^3: (256, 256, 384) coefficients <-> (256, 384, 384) grid along axis 1
     N, G = 256, 384
@@ -93,17 +85,10 @@ def main():
     c = torch.randn((N, N, G), dtype=torch.float64, device='cuda')
     g = torch.randn((N, G, G), dtype=torch.float64, device='cuda')
     gb = 8 * (c.numel() + g.numel()) / 1e9
-    arms = {f"P={p}": dict(DB_FFT_P=str(p)) for p in (8, 4)}
     print(f"\ny pass: n = {G}, M = {N}, outer = {N}, inner = {G}, {gb:.2f} GB per launch")
-    print(f"{'arm':18s} {'ms (median)':>12s} {'min':>8s} {'max':>8s} {'GB/s':>8s} {'CTAs/SM':>8s}")
-    for kind, label, make in ((0, "backward", lambda: (lambda: rf.backward(c, g, 1))), (1, "forward", lambda: (lambda: rf.forward(g, c, 1)))):
-        res = run_arms(arms, make)
-        for name, env in arms.items():
-            ms = statistics.median(res[name])
-            bps = lib._raw_db_rfft_blocks_per_sm(kind, G, N, 0, int(env['DB_FFT_P']))
-            out['y_pass'][f"{label} {name}"] = dict(ms=res[name], gbps=gb / (ms * 1e-3), blocks_per_sm=bps)
-            print(f"{label + ' ' + name:18s} {ms:12.3f} {min(res[name]):8.3f} {max(res[name]):8.3f} {gb / (ms * 1e-3):8.1f} {bps:8d}")
-    os.environ.pop("DB_FFT_P")
+    print(f"{'kernel':18s} {'ms (median)':>12s} {'min':>8s} {'max':>8s} {'GB/s':>8s} {'CTAs/SM':>8s}")
+    for kind, label, fn in ((0, "backward", lambda: rf.backward(c, g, 1)), (1, "forward", lambda: rf.forward(g, c, 1))):
+        out['y_pass'][label] = row(label, rounds(fn), gb, lib._raw_db_rfft_blocks_per_sm(kind, G, N, 0))
     if args.json:
         pathlib.Path(args.json).parent.mkdir(parents=True, exist_ok=True)
         pathlib.Path(args.json).write_text(json.dumps(out, indent=1))

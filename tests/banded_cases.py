@@ -1,10 +1,8 @@
-"""Shared bodies of the banded-solver tests: every selectable kernel variant (db_banded_set_mode 0 .. 3) on ragged batches against
-LAPACK (scipy.linalg.lapack dgbtrf / dgbtrs) and long-double products, through the CPU emulation of the kernels
-(tests/test_emu_banded.py) and on the GPU (tests/test_gpu_1b_banded.py).
+"""Shared bodies of the banded-solver tests: the combine / factor / solve / matvec kernels on ragged batches against LAPACK
+(scipy.linalg.lapack dgbtrf / dgbtrs) and long-double products, through the CPU emulation of the kernels (tests/test_emu_banded.py)
+and on the GPU (tests/test_gpu_1b_banded.py).
 
-The variants differ only in how data is loaded (bit 0: L2 loads in the factorisation; bit 1: factor columns read from global memory
-instead of through the cp.async ring of the solve), so their results must agree bit for bit.  The sizes cover every n around the ring
-depth (BS_DEPTH = 8 columns in flight), a warp's width, the largest per-m system of the 512 x 256 shallow-water problem (n = 1530) and
+The sizes cover every n from 1 to 9, a warp's width, the largest per-m system of the 512 x 256 shallow-water problem (n = 1530) and
 a batch past n = 1536, where the solve drops from 8 to 4 right-hand-side columns per CTA."""
 import ctypes as C
 import numpy as np
@@ -12,7 +10,6 @@ from scipy.linalg import lapack
 from dedalus_b200 import lib as dlib
 
 EPS = np.finfo(np.float64).eps
-MODES = (0, 1, 2, 3)
 NRHS_CYCLE = (1, 8, 9, 33)           # one column, exactly one chunk, one past a chunk, more than 32 columns in the row swap
 SMALL_NS = tuple(range(1, 10)) + (31, 32, 33, 100)
 
@@ -75,8 +72,8 @@ class Batch:
         return y, ya
 
 
-def _run(B, bt, mode, alias_x=False):
-    """combine -> factor -> solve -> matvec with kernel variant `mode`; returns host copies of lu, ipiv, x, ym, yl."""
+def _run(B, bt, alias_x=False):
+    """combine -> factor -> solve -> matvec; returns host copies of lu, ipiv, x, ym, yl."""
     lib, P = B.lib, B.ptr
     kl, ku, nsys = bt.kl, bt.ku, len(bt.ns)
     sysb = B.dev(np.frombuffer(bytes(bt.sys), dtype=np.uint8).copy())
@@ -86,18 +83,14 @@ def _run(B, bt, mode, alias_x=False):
     v1, v2 = B.dev(bt.v1), B.dev(bt.v2)
     x = v1 if alias_x else B.dev(np.full(bt.n_vec, np.nan))
     ym, yl = B.dev(np.full(bt.n_vec, np.nan)), B.dev(np.full(bt.n_vec, np.nan))
-    lib.call("db_banded_set_mode", mode)
-    try:
-        lib.call("db_banded_combine", P(sysb), nsys, kl, ku, bt.a0, P(m_d), bt.b0, P(l_d), P(lu), B.stream)
-        lu_comb = B.host(lu).copy()
-        lib.call("db_banded_factor", P(sysb), nsys, kl, ku, P(lu), P(ipiv), P(info), B.stream)
-        vc = dlib.VecComb(); vc.nvec = 2
-        vc.vec[0], vc.vec[1] = P(v1).value, P(v2).value
-        vc.coef[0], vc.coef[1] = bt.c1, bt.c2
-        lib.call("db_banded_solve", P(sysb), nsys, kl, ku, max(bt.ns), max(bt.nrhs), P(lu), P(ipiv), C.byref(vc), P(x), B.stream)
-        lib.call("db_banded_matvec", P(sysb), nsys, kl, ku, P(m_d), P(l_d), P(x), P(ym), P(yl), B.stream)
-    finally:
-        lib.call("db_banded_set_mode", -1)                 # back to the environment's choice (DB_BANDED_MODE, default 3)
+    lib.call("db_banded_combine", P(sysb), nsys, kl, ku, bt.a0, P(m_d), bt.b0, P(l_d), P(lu), B.stream)
+    lu_comb = B.host(lu).copy()
+    lib.call("db_banded_factor", P(sysb), nsys, kl, ku, P(lu), P(ipiv), P(info), B.stream)
+    vc = dlib.VecComb(); vc.nvec = 2
+    vc.vec[0], vc.vec[1] = P(v1).value, P(v2).value
+    vc.coef[0], vc.coef[1] = bt.c1, bt.c2
+    lib.call("db_banded_solve", P(sysb), nsys, kl, ku, max(bt.ns), max(bt.nrhs), P(lu), P(ipiv), C.byref(vc), P(x), B.stream)
+    lib.call("db_banded_matvec", P(sysb), nsys, kl, ku, P(m_d), P(l_d), P(x), P(ym), P(yl), B.stream)
     assert not B.host(info).any(), B.host(info)
     return dict(comb=lu_comb, lu=B.host(lu).copy(), ipiv=B.host(ipiv).copy(), x=B.host(x).copy(),
                 ym=B.host(ym).copy(), yl=B.host(yl).copy())
@@ -144,22 +137,15 @@ def _check_against_lapack(bt, r):
             assert np.all(np.abs(got - exact) <= (kl + ku + 2) * EPS * mag), (tag, name)
 
 
-def check_banded_variants(B, kl, ku, ns, nrhs, seed=0, alias=True):
-    """Every kernel variant on one ragged batch: LAPACK-accurate in each, and bitwise identical across variants (a race in one
-    load path corrupts a value and cannot hide behind a tolerance).  With `alias`, x is also solved in place over a right-hand-side
-    vector, which the ABI allows: each CTA stages its right-hand-side columns in shared memory before it writes any of x."""
+def check_banded(B, kl, ku, ns, nrhs, seed=0, alias=True):
+    """One ragged batch, LAPACK-accurate.  With `alias`, x is also solved in place over a right-hand-side vector, which the ABI
+    allows: each CTA stages its right-hand-side columns in shared memory before it writes any of x; the result must be bitwise equal."""
     bt = Batch(ns, nrhs, kl, ku, seed)
-    runs = {mode: _run(B, bt, mode) for mode in MODES}
-    _check_against_lapack(bt, runs[MODES[0]])
-    for mode in MODES[1:]:
-        for key in ("comb", "lu", "ipiv", "x", "ym", "yl"):
-            a, b = runs[MODES[0]][key], runs[mode][key]
-            assert a.tobytes() == b.tobytes(), (dict(kl=kl, ku=ku, mode=mode), key,
-                                                _first_difference(bt, a, b) if key == "x" else None)
+    run = _run(B, bt)
+    _check_against_lapack(bt, run)
     if alias:
-        for mode in MODES:
-            r = _run(B, bt, mode, alias_x=True)
-            assert r["x"].tobytes() == runs[mode]["x"].tobytes(), (mode, "x solved over v1", _first_difference(bt, r["x"], runs[mode]["x"]))
+        r = _run(B, bt, alias_x=True)
+        assert r["x"].tobytes() == run["x"].tobytes(), ("x solved over v1", _first_difference(bt, r["x"], run["x"]))
 
 
 def _first_difference(bt, a, b):
@@ -170,24 +156,3 @@ def _first_difference(bt, a, b):
         s = bt.sys[i]
         if s.vec_off <= bad[0] < s.vec_off + s.n * s.nrhs:
             return dict(system=i, n=s.n, nrhs=s.nrhs)
-
-
-def check_shallow_water_modes(g, steps=3):
-    """The stock shallow-water problem (16 x 8, RK222): the ring solve (variant 0) and the default (variant 3) leave bitwise-equal
-    states after `steps` steps."""
-    import sphere_cases as S
-    from dedalus_b200.lib import get_lib
-    lib = get_lib()
-    states = {}
-    for mode in (0, 3):
-        lib.call("db_banded_set_mode", mode)
-        try:
-            sw, solver, _, dt = S.run_shallow_water(g, "sw16")
-            for _ in range(steps):
-                solver.step(dt)
-            states[mode] = {name: np.array(sw[name]['c']) for name in ('u', 'h')}
-            assert solver.bset.last_verify < 1e-12, (mode, solver.bset.last_verify)
-        finally:
-            lib.call("db_banded_set_mode", -1)
-    for name in ('u', 'h'):
-        assert states[0][name].tobytes() == states[3][name].tobytes(), (name, np.abs(states[0][name] - states[3][name]).max())

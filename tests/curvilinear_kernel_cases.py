@@ -465,7 +465,7 @@ def mmt_apply(B, mat, x, expect, offset=None):
     md, xd, od = B.dev_at(mat, offset == "mat"), B.dev_at(x, offset == "in"), B.dev_at(_nan((outer, m, inner)), offset == "out")
     ptrs = [B.ptr(t).value for t in (md, xd, od)]
     aligned = all(p % 16 == 0 for p in ptrs)
-    rule = aligned and n % 2 == 0 and inner % 2 == 0 and os.environ.get("DB_MMT_DMMA", "1") != "0"
+    rule = aligned and n % 2 == 0 and inner % 2 == 0
     assert rule == (expect == "dmma"), (dict(m=m, n=n, inner=inner, aligned=aligned), expect)
     before = B.lib._raw_db_mmt_dmma_launches()
     B.lib.call("db_mmt_apply", ptrs[0], m, n, ptrs[1], ptrs[2], outer, inner, B.stream)

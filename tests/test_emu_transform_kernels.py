@@ -31,14 +31,6 @@ def test_rfft_register(n, M, outer, inner):
     assert K.check_rfft(B, n, M, outer, inner, derivs=(0, 1, 2, 3, 4)) is True
 
 
-@pytest.mark.parametrize("n", [192, 384])
-def test_rfft_register_tile_pairs_4(n):
-    """DB_FFT_P = 4 (read at every launch at n = 192, 384): half-height tiles."""
-    with K.env(DB_FFT_P=4):
-        for M in (2, 2 * n // 3):
-            assert K.check_rfft(B, n, M, 1, 48, derivs=(0, 2, 4), path="regs P=4") is True
-
-
 def test_rfft_register_many_tiles_per_cta():
     """inner = 16 * 20 at n = 48: 20 tiles per outer index and 3 outer indices walk through the persistent CTAs (one SM here)."""
     assert K.check_rfft(B, 48, 32, 3, 320, derivs=(0, 3), impulse=False) is True
@@ -108,21 +100,6 @@ def test_band_lines(n, lines, npre, stride):
     K.check_band_lines(B, n, lines, npre, stride)
 
 
-_CHEB_P_SUB = "DB_CHEB_P_SUBPROCESS"
-
-
-@pytest.mark.parametrize("P", [2, 8])
-def test_cheb_tile_pairs(P):
-    """DB_CHEB_P = 2 and 8 (read once per process: a subprocess each) at n = 192, 384: the register Chebyshev tiles at both heights."""
-    if os.environ.get(_CHEB_P_SUB):
-        pytest.skip("runs in its own subprocess")
-    cmd = [sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", __file__, "-k", "cheb_register and (192 or 384)"]
-    out = subprocess.run(cmd, capture_output=True, text=True, timeout=1200, env=dict(os.environ, DB_CHEB_P=str(P), **{_CHEB_P_SUB: "1"}),
-                         cwd=str(ROOT))
-    assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-2000:]
-    assert " passed" in out.stdout and "failed" not in out.stdout
-
-
 # ---- blocked and peer entries
 @pytest.mark.parametrize("n_peers", [1, 2, 3, 4, 8])
 @pytest.mark.parametrize("in_blocked", [False, True])
@@ -150,10 +127,12 @@ def test_x_products_schedules(sched):
         K.check_x_products(B, 48, 30, 64, sched, in_pad=10, out_pad=6, impulse=impulse)
 
 
-@pytest.mark.parametrize("P", [4, 8])
-def test_x_products_tile_pairs(P):
-    K.check_x_products(B, 192, 128, 32, "three_held", P=P, in_pad=2, out_pad=4)
-    K.check_x_products(B, 384, 254, 16, "held_reuse", P=P, impulse=True)
+@pytest.mark.parametrize("n", [192, 384])
+def test_x_products_long_lines(n):
+    if n == 192:
+        K.check_x_products(B, 192, 128, 32, "three_held", in_pad=2, out_pad=4)
+    else:
+        K.check_x_products(B, 384, 254, 16, "held_reuse", impulse=True)
 
 
 def test_x_products_rejections():
@@ -169,11 +148,8 @@ def test_x_products_supported_agrees():
 def test_register_kernels_under_other_schedules(env):
     """The register kernels and the fused x pass with threads and blocks in descending order, and with their cp.async copies landing
     at issue (a staging buffer refilled while it is still being read would show)."""
-    if os.environ.get(_CHEB_P_SUB):
-        pytest.skip("runs in its own subprocess")
     cmd = [sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", __file__, "-k",
            "(rfft_register and 96) or x_products_schedules or cheb_register and 96 or many_tiles"]
-    out = subprocess.run(cmd, capture_output=True, text=True, timeout=1200, env=dict(os.environ, **env, **{_CHEB_P_SUB: "1"}),
-                         cwd=str(ROOT))
+    out = subprocess.run(cmd, capture_output=True, text=True, timeout=1200, env=dict(os.environ, **env), cwd=str(ROOT))
     assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-2000:]
     assert " passed" in out.stdout and "failed" not in out.stdout

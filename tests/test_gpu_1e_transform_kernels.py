@@ -22,13 +22,6 @@ def test_rfft_register(n, M, outer, inner):
     assert K.check_rfft(B, n, M, outer, inner, derivs=(0, 1, 2, 3, 4)) is True
 
 
-@pytest.mark.parametrize("n", [192, 384])
-def test_rfft_register_tile_pairs_4(n):
-    with K.env(DB_FFT_P=4):
-        for M in (2, 2 * n // 3):
-            assert K.check_rfft(B, n, M, 1, 48, derivs=(0, 2, 4), path="regs P=4") is True
-
-
 @pytest.mark.parametrize("n,M", [(96, 64), (384, 256)])
 def test_rfft_register_persistent_grid_extremes(n, M):
     """The persistent grid with a single tile (inner = 16: one CTA), and with 4 tiles per SM (inner = 16 * SMs * 4)."""
@@ -127,19 +120,21 @@ def test_x_products_schedules(sched):
         K.check_x_products(B, 48, 30, 64, sched, in_pad=10, out_pad=6, impulse=impulse)
 
 
-@pytest.mark.parametrize("P", [4, 8])
-def test_x_products_tile_pairs(P):
-    K.check_x_products(B, 192, 128, 32, "three_held", P=P, in_pad=2, out_pad=4)
-    K.check_x_products(B, 384, 254, 16, "held_reuse", P=P, impulse=True)
-    # many more tiles than the persistent grid has CTAs
-    K.check_x_products(B, 96, 64, 16 * B.sms * 6, "three_held", P=P, in_pad=2, out_pad=2)
+@pytest.mark.parametrize("case", ["192", "384", "many_tiles"])
+def test_x_products_long_lines(case):
+    if case == "192":
+        K.check_x_products(B, 192, 128, 32, "three_held", in_pad=2, out_pad=4)
+    elif case == "384":
+        K.check_x_products(B, 384, 254, 16, "held_reuse", impulse=True)
+    else:                                               # many more tiles than the persistent grid has CTAs
+        K.check_x_products(B, 96, 64, 16 * B.sms * 6, "three_held", in_pad=2, out_pad=2)
 
 
-@pytest.mark.parametrize("P", [4, 8])
-def test_x_products_benchmark_shape(P):
-    """The x-line length and coefficient count of the 256^3 benchmark (n = 384, M = 256) with three held factors over 49152 lines,
-    checked on a sample of line pairs."""
-    K.check_x_products_large(B, 384, 256, 192 * 256, "three_held", P=P, sample=96)
+@pytest.mark.parametrize("sched", ["three_held", "held_reuse"])
+def test_x_products_benchmark_shape(sched):
+    """The x-line length and coefficient count of the 256^3 benchmark (n = 384, M = 256) over 49152 lines, checked on a sample of
+    line pairs: the benchmark's schedule (three held factors) and one that reuses a held factor."""
+    K.check_x_products_large(B, 384, 256, 192 * 256, sched, sample=96)
 
 
 def test_x_products_rejections():

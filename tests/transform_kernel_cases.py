@@ -889,7 +889,7 @@ def x_products(B, n, cin, items, n_out, kscale, n_held, in_pad=0, out_pad=0, exp
     return h[:, :M * inner].reshape(n_out, M, inner), h[:, M * inner:], d
 
 
-def check_x_products(B, n, M, inner, sched, P=None, in_pad=0, out_pad=0, impulse=False, seed=0, kscale=1.1):
+def check_x_products(B, n, M, inner, sched, in_pad=0, out_pad=0, impulse=False, seed=0, kscale=1.1):
     n_in, n_out, rec = xprod_schedules()[sched]
     items = xprod_items(rec)
     n_held = len({r[3] for r in rec if r[6] & HELD})
@@ -903,8 +903,7 @@ def check_x_products(B, n, M, inner, sched, P=None, in_pad=0, out_pad=0, impulse
     else:
         cin = rng.standard_normal((n_in, M, inner))
     cin[:, 1, :] = 1e3                                    # the sin(0) slot is not read
-    with env(DB_XPROD_P=P):
-        got, gaps, d = x_products(B, n, cin, items, n_out, kscale, n_held, in_pad, out_pad)
+    got, gaps, d = x_products(B, n, cin, items, n_out, kscale, n_held, in_pad, out_pad)
     assert d == 1
     assert np.isnan(gaps).all(), "wrote into the padding between outputs"
     refs = xprod_ref(cin, n, items, kscale, n_out)
@@ -935,7 +934,7 @@ def check_x_products_rejections(B):
 
 
 def check_x_products_supported_agrees(B):
-    """RealFourierTransform.x_products_supported against the C entry point (rejection or launch) over (n, M, inner, n_held, P)."""
+    """RealFourierTransform.x_products_supported against the C entry point (rejection or launch) over (n, M, inner, n_held)."""
     from dedalus_b200.transforms import RealFourierTransform
     _, _, rec = xprod_schedules()["linear_no_held"]
     items = xprod_items(rec)
@@ -944,24 +943,21 @@ def check_x_products_supported_agrees(B):
         for M in (2, 2 * n // 3 - 1, 2 * n // 3, 2 * n // 3 + 2):
             for inner in (8, 16, 24, 32):
                 for n_held in (0, 3, 4):
-                    for P in (4, 8):
-                        with env(DB_XPROD_P=P):
-                            ok = RealFourierTransform(n, M).x_products_supported(inner, n_held)
-                            _, _, d = x_products(B, n, np.zeros((3, M, inner)), items, 3, 1.0, n_held, expect_rc=0 if ok else 1)
-                        assert d == (1 if ok else 0)
-                        seen.add(ok)
+                    ok = RealFourierTransform(n, M).x_products_supported(inner, n_held)
+                    _, _, d = x_products(B, n, np.zeros((3, M, inner)), items, 3, 1.0, n_held, expect_rc=0 if ok else 1)
+                    assert d == (1 if ok else 0)
+                    seen.add(ok)
     assert seen == {True, False}
 
 
-def check_x_products_large(B, n, M, inner, sched, P=None, sample=64, seed=0, kscale=1.0):
+def check_x_products_large(B, n, M, inner, sched, sample=64, seed=0, kscale=1.0):
     """The fused x pass over `inner` lines; the reference on `sample` random line pairs (the bound pairs lines 2m, 2m + 1)."""
     n_in, n_out, rec = xprod_schedules()[sched]
     items = xprod_items(rec)
     n_held = len({r[3] for r in rec if r[6] & HELD})
     rng = np.random.default_rng(seed + n + inner)
     cin = rng.standard_normal((n_in, M, inner))
-    with env(DB_XPROD_P=P):
-        got, gaps, d = x_products(B, n, cin, items, n_out, kscale, n_held)
+    got, gaps, d = x_products(B, n, cin, items, n_out, kscale, n_held)
     assert d == 1
     pairs = np.sort(rng.choice(inner // 2, sample, replace=False))
     cols = np.stack([2 * pairs, 2 * pairs + 1], 1).reshape(-1)
