@@ -66,7 +66,9 @@ def test_cfl_controller_matches_reference(golden):
 @pytest.mark.parametrize("timestepper", list(d3.schemes.keys()) + ["RKGFY"])
 def test_heat_periodic_every_timestepper(timestepper):
     """Reference integration test tests/test_ivp.py:18-49 (1-D heat equation, every scheme in `schemes`, 20 steps,
-    analytic solution), here on the real Fourier basis: dt(u) - dx(dx(u)) = F, F = sin(x)."""
+    analytic solution), here on the real Fourier basis: dt(u) - dx(dx(u)) = F, F = sin(x).  A consistency check only (1 x 1 and 2 x 2
+    systems, a solution of 2e-4, default allclose tolerances): the device step of every scheme is checked against a long-double
+    replay in test_emu_timesteps.py / test_gpu_1g_timesteps.py."""
     from dedalus_b200 import timesteppers as ts
     scheme = ts.schemes.get(timestepper, getattr(ts, timestepper))
     c = d3.Coordinate('x')
